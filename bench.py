@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the OMG two-stage SDXL denoising hot path (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is ONE IMAGE through the whole hot path as the reference executes it (config 2): stage 1 (30 steps, main
 UNet B=4) + stage 2 (30 steps, main UNet B=4, and for step index > 15 two concept UNets B=2 with un-merged LoRA) =
@@ -15,6 +15,9 @@ UNet B=4) + stage 2 (30 steps, main UNet B=4, and for step index > 15 two concep
   sum(algorithmic FLOPs) / sum(durations).
 * cpu_baseline: the fp32 oracle (a port of the reference's diffusers path) timed on the host cores for one
   sample-forward at the same latent size, extrapolated to images/sec (= 1 / (296 * t)).
+* --dump-outputs DIR: the final latents of both stages of the last timed image (what the pipeline call returns),
+  written as DIR/stage1_latents.npy and DIR/stage2_latents.npy in float32.  Weights, prompts, masks and noise come
+  from fixed seeds, so two builds run with the same arguments can be compared output for output.
 N > 1: independent images, one replica per GPU (weights broadcast once over NCCL, final latents all-gathered);
 scaling is weak (K images per GPU).
 """
@@ -43,8 +46,19 @@ def read_peaks():
         return None
 
 
+def gpu_identity(index):
+    """Name and power limit of the card the numbers were measured on."""
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        name, watts = [x.strip() for x in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(watts)}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -167,7 +181,7 @@ def workload_config(n_gpus, total_images=0):
                         "7.5, prompt-to-prompt AttentionReplace(50, cross 1.0, self 0.4), as-executed 296 UNet "
                         "sample-forwards per image",
             "images_per_gpu_per_step": 1, "parallelism": f"dp{n_gpus} (independent images, weight replicas)",
-            "l2_policy": "inputs+weights (5.1 GB) exceed the 126 MB L2; no flush needed between steps"}
+            "l2_policy": "inputs+weights (5.1 GB) exceed the 50 MB L2; no flush needed between steps"}
 
 
 class StdoutToStderr:
@@ -201,6 +215,8 @@ def _main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--skip-e2e", action="store_true", help="profile runs only: do not repeat the timed region with host buffers")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final latents of the last timed image as float32 .npy files into DIR")
     ap.add_argument("--total-images", type=int, default=0,
                     help="BASELINE config 5: this many independent images (seeds 0..N-1) sharded image j -> rank j mod G "
                          "(strong scaling); overrides --steps")
@@ -328,6 +344,11 @@ def _main():
         gathered = [torch.empty_like(mine) for _ in range(world)]
         dist.all_gather(gathered, mine)
     finite = all(bool(torch.isfinite(o[1]).all()) for o in outs)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in zip(("stage1_latents", "stage2_latents"), outs[-1]):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.float().cpu().numpy())
 
     if rank == 0:
         imgs = args.total_images if args.total_images else args.steps * world
@@ -364,13 +385,7 @@ def _main():
         g_flops = sum(p[0] for p in prof)
         g_ms = sum(p[1].elapsed_time(p[2]) for p in prof)
         achieved = g_flops / g_ms / 1e9 if g_ms > 0 else 0.0
-        peak = peaks["bf16_tflops_sustained"] if peaks else 1400.0
-        traffic = None
-        try:  # measured DRAM bytes per launch of the same forward (ncu launch list committed under profiles/)
-            from scripts.summarize_launches import summarize
-            n_l, traffic = summarize(os.path.join(ROOT, "profiles", "r02_launches_main_unet_b4.csv"), os.devnull, "")
-        except Exception:
-            traffic = None
+        peak = peaks["bf16_tflops_sustained"] if peaks else 989.0  # H100 SXM data sheet, dense FP16 (700 W card)
         flops_img = SAMPLE_FORWARDS_PER_IMAGE * unet_flops(cfg, IMAGE // 8, IMAGE // 8)
         out = {
             "metric": "1024^2 images/sec @30 steps, 2 concepts", "value": value, "unit": "images/sec",
@@ -378,15 +393,14 @@ def _main():
             "higher_is_better": True, "scaling": "strong" if args.total_images else "weak", "vs_baseline": None,
             "dtype": "f16", "data": "synthetic", "config": workload_config(world, args.total_images),
             "e2e": {"value": None if args.skip_e2e else e2e, "unit": "images/sec", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
-            "gpu_launches": launches, "clocks": clocks,
+            "gpu_launches": launches, "clocks": clocks, "gpu": gpu_identity(local),
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": achieved / peak, "traffic": traffic, "kernel": "gemm_tc_kernel",
-                         "traffic_note": "dram__bytes_read+write per launch, mean over the 488 gemm_tc_kernel launches of one "
-                                         "main-UNet forward, ncu cold-cache pass (profiles/r02_launches_main_unet_b4.csv)",
+                         "frac": achieved / peak, "kernel": "gemm_tc_kernel",
                          "algorithmic_bytes_per_launch": sum(p[3] for p in prof) / max(len(prof), 1),
                          "algorithmic_flops_per_launch": g_flops / max(len(prof), 1),
                          "launches_profiled": len(prof),
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "fallback"},
+                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks
+                                        else "H100 SXM data sheet (dense FP16), not a measured rate"},
             "unet_step_ms": {"main_b4": None},
             "whole_path_tflops": flops_img * imgs / (ms / 1e3) / 1e12 / world,
             "weight_broadcast_s": t_bcast, "finite": finite,

@@ -1,5 +1,5 @@
 /*
- * omg_b200 — C ABI of the B200-native OMG denoising hot path.
+ * omg_b200 — C ABI of the H100-native (sm_90a) OMG denoising hot path.
  *
  * The reference (kongzhecn/OMG) is pure Python on diffusers and has no FFI of its own; the
  * "interface each entry point replaces" is therefore the torch / diffusers / xformers library call
@@ -44,7 +44,7 @@ enum { OMG_EPI_NONE = 0, OMG_EPI_GEGLU = 1, OMG_EPI_SILU = 2, OMG_EPI_QUICK_GELU
  *
  * Replaces: torch.nn.Linear / Conv2d(3x3 | 1x1, stride 1 | 2) / peft LoRA delta / GEGLU inside
  * diffusers UNet2DConditionModel.forward, reference call sites src/pipelines/lora_pipeline.py:546-566,592-599
- * (cuBLAS / cuDNN in the reference).  tcgen05 tensor cores, TMA-staged operands.
+ * (cuBLAS / cuDNN in the reference).  wgmma tensor cores, TMA-staged operands.
  * OMG_EPI_GEGLU: W rows (and bias) are interleaved (value_j, gate_j) pairs; out has N/2 channels,
  * out_j = value_j * gelu_erf(gate_j).   OMG_EPI_SILU: epi(x) = x * sigmoid(x) (time-embedding MLPs).
  * OMG_EPI_QUICK_GELU: x * sigmoid(1.702 x), OMG_EPI_GELU: erf-gelu (the fc1 activations of the two CLIP text towers,
@@ -66,7 +66,7 @@ typedef struct {
     const void* residual; /* contiguous [B*H*W, residual_ld] fp16 or NULL, added after the epilogue */
     int32_t residual_ld;
     int32_t epilogue;
-    int32_t block_n;    /* 0 = auto; else 64 | 128 | 160 | 256 */
+    int32_t block_n;    /* 0 = auto; else 64 | 128 | 160 | 256 | 320 */
     /* LayerNorm folded into a GEMM pair (BasicTransformerBlock norm1/2/3 [3P] followed by to_q|k|v / ff.net.0.proj):
      * the GEMM that PRODUCES the hidden state h writes per-row partial (sum, sum of squares) of its output, one
      * partial per n-tile, to row_stats_out [n_tiles][rows][2] fp32; the GEMM that CONSUMES LayerNorm(h) runs on raw h
@@ -87,7 +87,7 @@ typedef struct {
     int64_t col_group_end[8];
     int32_t w_group_planes; /* 0: one weight matrix for all rows; else == n_col_groups: w is [planes][N][Ktot] and row
                              * group g multiplies with plane g (per-stream weights, e.g. W + s B_g A_g merged per concept) */
-    int32_t cta_pair;   /* 0 = auto, 1 = single-CTA tiles, 2 = CTA pairs (cta_group::2, 256 x block_n tiles; block_n 256 | 160),
+    int32_t cta_pair;   /* 0 = auto, 1 = single 128-row tiles, 2 = not available (rejected),
                          * 3 = tall tiles (one CTA, 256 x 160: two 128-row sub-tiles share each weight tile; block_n 160) */
     /* GroupNorm statistics out of the producing GEMM / conv (ResnetBlock2D norm1/norm2, Transformer2DModel.norm,
      * conv_norm_out [3P]): per image and per 32-pixel block of the output, the per-channel (sum, sum of squares) of the
@@ -265,7 +265,7 @@ int omg_plan_run(const omg_plan* plan, void* stream);
 
 /* Error string of the last failing call on this thread (never NULL). */
 const char* omg_last_error(void);
-/* Library / build identification: returns e.g. "omg_b200 sm_100a". */
+/* Library / build identification: returns e.g. "omg_b200 0.1 sm_90a". */
 const char* omg_version(void);
 /* Number of kernel launches issued by this library since process start (bench.py's gpu_launches). */
 uint64_t omg_launch_count(void);

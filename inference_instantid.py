@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""OMG + InstantID multi-identity generation on the B200 path.  The reference CLI's flags (names, defaults, types:
+"""OMG + InstantID multi-identity generation on the H100 path.  The reference CLI's flags (names, defaults, types:
 inference_instantid.py:259-286, pinned by tests/golden/cli_flags.json), prompt mini-DSL, two-stage flow and output
 files; additions (non-breaking): --synthetic, --tiny, --num_inference_steps, --image_size, --dedup, --mask_boxes,
 --face_embeds, --face_kps.
@@ -196,7 +196,7 @@ def build_synthetic(args, device):
 if __name__ == "__main__":
     args = parse_args()
     if not torch.cuda.is_available():
-        raise SystemExit("the B200 path needs a CUDA device (there is no CPU fallback)")
+        raise SystemExit("the H100 path needs a CUDA device (there is no CPU fallback)")
     device = torch.device("cuda")
     from omg_b200 import synthetic
     size = args.image_size

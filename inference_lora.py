@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""OMG + LoRA multi-concept generation on the B200 path.  Same flags, prompt mini-DSL, two-stage flow and output
+"""OMG + LoRA multi-concept generation on the H100 path.  Same flags, prompt mini-DSL, two-stage flow and output
 files as the reference CLI (inference_lora.py:201-323); additions (non-breaking): --synthetic, --num_inference_steps,
 --image_size, --mask_boxes, --vae_fp16_safe.
 
@@ -141,7 +141,7 @@ def build_model_sd(args, prompts, device):
 if __name__ == "__main__":
     args = parse_args()
     if not torch.cuda.is_available():
-        raise SystemExit("the B200 path needs a CUDA device (there is no CPU fallback)")
+        raise SystemExit("the H100 path needs a CUDA device (there is no CPU fallback)")
     device = torch.device("cuda")
     prompts = [args.prompt] * 2
     width = height = args.image_size

@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI library (nvcc, sm_100a only).  Used by __graft_entry__.build()."""
+"""In-tree build of the C-ABI library (nvcc, sm_90a only).  Used by __graft_entry__.build()."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libomg_b200.so")
 OBJ_DIR = os.path.join(HERE, "..", "build", "obj")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -53,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(compile_one, jobs))
     if jobs or not os.path.exists(LIB_PATH):
-        r = subprocess.run([nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"],
+        r = subprocess.run([nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a"],
                            capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

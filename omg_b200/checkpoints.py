@@ -196,7 +196,7 @@ def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfi
         return out
 
     if strict and skipped:
-        raise ValueError(f"{len(skipped)} LoRA tensors target modules the B200 path does not adapt, e.g. {skipped[:3]}")
+        raise ValueError(f"{len(skipped)} LoRA tensors target modules this path does not adapt, e.g. {skipped[:3]}")
     unet_lora = finish(parts)
     shapes = {n: (i, o) for n, i, o in lora_target_names(cfg)}
     for name, (A, B, _s) in unet_lora.items():

@@ -115,5 +115,5 @@ extern "C" int omg_plan_run(const omg_plan* plan, void* stream) {
 }
 
 extern "C" const char* omg_last_error(void) { return omg::g_err; }
-extern "C" const char* omg_version(void) { return "omg_b200 0.1 sm_100a"; }
+extern "C" const char* omg_version(void) { return "omg_b200 0.1 sm_90a"; }
 extern "C" uint64_t omg_launch_count(void) { return omg::g_launches.load(); }

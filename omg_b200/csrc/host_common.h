@@ -46,10 +46,9 @@ bool plan_recording();
 void plan_note(std::function<int(void*)> step);
 
 // Every kernel of this library can be launched with programmatic dependent launch (PDL): the next kernel's CTAs may
-// become resident and run their prologue (barrier init, TMEM alloc, descriptor prefetch) while the previous kernel
-// drains; each kernel executes griddepcontrol.wait before its first dependent global access.  Measured on the full
-// two-stage loop inside CUDA graphs: 2791.8 ms/image with the attribute, 2770.4 ms without (no gain: the one-CTA-per-
-// SM kernels cannot co-reside anyway), so it is opt-in: OMG_PDL=1.
+// become resident and run their prologue (barrier init, descriptor prefetch) while the previous kernel drains; each
+// kernel executes griddepcontrol.wait before its first dependent global access.  Opt-in (OMG_PDL=1): the one-CTA-per-SM
+// GEMM cannot co-reside with its predecessor anyway.
 bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>

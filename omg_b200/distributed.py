@@ -1,7 +1,7 @@
 """Data-parallel plumbing for independent images (SURVEY section 8e): every image (seed) is an independent two-stage
 trajectory, so images are sharded round-robin over ranks with NO collective inside the denoising loop.  The only
 collectives are one broadcast of the weights from rank 0 at start-up and one all-gather of the final latents
-(128 KiB per image).  torch.distributed (NCCL over NVLink on the B200 box, gloo in the CPU tests) is the transport."""
+(128 KiB per image).  torch.distributed (NCCL over NVLink between GPUs, gloo in the CPU tests) is the transport."""
 from typing import Dict, List
 
 import torch

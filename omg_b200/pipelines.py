@@ -1,4 +1,4 @@
-"""The two-stage OMG denoising pipelines on the B200 kernels, behind the reference call surface.
+"""The two-stage OMG denoising pipelines on the H100 kernels, behind the reference call surface.
 
   LoraMultiConceptPipeline        <- src/pipelines/lora_pipeline.py:154-681
   InstantidMultiConceptPipeline   <- src/pipelines/instantid_pipeline.py:157-767

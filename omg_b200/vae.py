@@ -1,4 +1,4 @@
-"""SDXL VAE decoder on the B200 kernels (SURVEY 8f-1: the step right after the denoising loop,
+"""SDXL VAE decoder on the H100 kernels (SURVEY 8f-1: the step right after the denoising loop,
 src/pipelines/lora_pipeline.py:634-661: `image = vae.decode(latents / scaling_factor)` + postprocess).
 
 Everything runs through the same C-ABI kernels as the UNet: channels-last fp16 activations, 3x3 convs as implicit
@@ -106,7 +106,7 @@ class PackedVaeDecoder:
     def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: VaeConfig = VaeConfig(), device="cuda"):
         self.cfg, self.device = cfg, torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("the B200 path needs a CUDA device (there is no CPU fallback)")
+            raise RuntimeError("the H100 path needs a CUDA device (there is no CPU fallback)")
         sd = {k: v.float() for k, v in state_dict.items() if k.startswith(("decoder.", "post_quant_conv."))}
         dev, p = self.device, {}
         self.p = p

@@ -9,10 +9,7 @@ import os
 import subprocess
 import sys
 
-VARIANTS = [("default", {}), ("gn_stats_pass", {"OMG_GN_FUSE": "0"}),
-            ("cross_per_head_ctas", {"OMG_ATTN_CROSS": "0"}), ("trunk_fp32_twins", {"OMG_TRUNK_F32": "1"}),
-            ("attn_per_tile_ctas", {"OMG_ATTN_PERSISTENT": "0"}),
-            ("r01_equivalent", {"OMG_GN_FUSE": "0", "OMG_ATTN_CROSS": "0", "OMG_ATTN_PERSISTENT": "0"}),
+VARIANTS = [("default", {}), ("gn_stats_pass", {"OMG_GN_FUSE": "0"}), ("trunk_fp32_twins", {"OMG_TRUNK_F32": "1"}),
             ("launch_plan_executor", {"OMG_EXECUTOR": "plan"})]
 if "--variants" in sys.argv:
     want = sys.argv[sys.argv.index("--variants") + 1].split(",")

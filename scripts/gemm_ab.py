@@ -1,4 +1,4 @@
-"""Tall 256x160 tiles vs 256x320 CTA-pair tiles on the narrow-N GEMM / conv shapes of the SDXL UNet (B=4):
+"""Tall 256x160 tiles vs 128x320 tiles on the narrow-N GEMM / conv shapes of the SDXL UNet (B=4):
 median of 20 timed launches each, L2 flushed between launches.  One JSON line per shape."""
 import json
 import sys
@@ -38,7 +38,7 @@ for (M, N, K, tag) in [(4096, 1280, 1280, "out1280"), (4096, 1280, 5120, "ff2_12
     x, w, res = rnd(M, K), rnd(N, K, scale=K ** -0.5), rnd(M, N)
     out = torch.empty(M, N, device=dev, dtype=torch.float16)
     r = {"name": tag, "gflop": 2.0 * M * N * K / 1e9}
-    for name, kw in (("tall160", dict(block_n=160, cta_pair=3)), ("pair320", dict(block_n=320)), ("pair256", dict(block_n=256, cta_pair=2))):
+    for name, kw in (("tall160", dict(block_n=160, cta_pair=3)), ("pair320", dict(block_n=320))):
         ms = timeit(lambda: ops.linear(x, w, residual=res, out=out, **kw))
         r[name] = {"us": round(ms * 1e3, 1), "tflops": round(r["gflop"] / ms, 1)}
     print(json.dumps(r), flush=True)

@@ -1,4 +1,4 @@
-"""Per-kernel timing on the B200 (CUDA events, L2 flushed between iterations) for the SDXL shapes of the hot path,
+"""Per-kernel timing on the GPU (CUDA events, L2 flushed between iterations) for the SDXL shapes of the hot path,
 next to the torch library call (cuBLAS / cuDNN / SDPA) the reference would make.  Prints TFLOP/s and GB/s."""
 import json
 import sys
@@ -70,15 +70,6 @@ for (M, N, K, tag) in [(16384, 1920, 640, "qkv640"), (16384, 640, 640, "out640")
         ms = timeit(lambda: ops.linear(x, wi, out=o2, epilogue=1))
         report(f"geglu_{tag}", ms, 2.0 * M * N * K, ref_ms=ref)
 
-# ---- CTA pairs (cta_group::2) vs single-CTA tiles, block_n 256
-for (M, N, K, tag) in [(16384, 1920, 640, "qkv640"), (16384, 5120, 640, "ff1_640"), (4096, 3840, 1280, "qkv1280"),
-                       (4096, 10240, 1280, "ff1_1280"), (8192, 10240, 1280, "ff1_1280_b8"), (8192, 1280, 5120, "ff2_1280_b8"),
-                       (16384, 640, 2560, "ff2_640")]:
-    x, w = rnd(M, K), rnd(N, K, scale=K ** -0.5)
-    out = torch.empty(M, N, device=dev, dtype=torch.float16)
-    for cp in (1, 2):
-        ms = timeit(lambda: ops.linear(x, w, out=out, block_n=256, cta_pair=cp))
-        report(f"pair{cp}_{tag}", ms, 2.0 * M * N * K)
 for (M, N, K, tag) in [(4096, 1280, 1280, "out1280"), (4096, 1280, 5120, "ff2_1280"), (8192, 1280, 5120, "ff2_1280_b8"),
                        (8192, 1280, 1280, "out1280_b8"), (16384, 640, 2560, "ff2_640")]:
     x, w = rnd(M, K), rnd(N, K, scale=K ** -0.5)

@@ -65,9 +65,9 @@ def lin(M, N, K, epi=L.EPI_NONE, residual=False):
     return lambda: ops.linear(x, w, bias=bias, residual=res, out=out, epilogue=epi)
 
 
-cases.append(("ff1 GEGLU 4096x10240x1280 (CTA pair)", lin(4096, 10240, 1280, L.EPI_GEGLU)))
+cases.append(("ff1 GEGLU 4096x10240x1280 (128 x 256 tiles)", lin(4096, 10240, 1280, L.EPI_GEGLU)))
 cases.append(("ff2 4096x1280x5120 +residual (tall tile)", lin(4096, 1280, 5120, residual=True)))
-cases.append(("qkv 4096x3840x1280 (CTA pair)", lin(4096, 3840, 1280)))
+cases.append(("qkv 4096x3840x1280", lin(4096, 3840, 1280)))
 cases.append(("out-proj 4096x1280x1280 +residual (tall tile)", lin(4096, 1280, 1280, residual=True)))
 cases.append(("ff1 GEGLU 16384x5120x640", lin(16384, 5120, 640, L.EPI_GEGLU)))
 

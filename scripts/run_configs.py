@@ -1,4 +1,4 @@
-"""BASELINE.json configs 3, 4 on one B200 (config 2 is bench.py's workload, config 5 its --gpus sweep).
+"""BASELINE.json configs 3, 4 on one GPU (config 2 is bench.py's workload, config 5 its --gpus sweep).
 
   (config 1, the full-width parity check against the fp32 oracle, is tests/test_config1_gpu.py)
   config 3  OMG + InstantID, 2 identities (IP-adapter concept UNet + IdentityNet), 1024^2, 30 steps: s / image.

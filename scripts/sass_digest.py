@@ -1,5 +1,5 @@
-"""Opcode digest of the shipped library: per kernel, how many tcgen05 / TMA / TMEM / mbarrier SASS instructions it holds
-(cuobjdump -sass), plus the proof of absence of the legacy tensor-core paths (HMMA / wgmma).  Written to
+"""Opcode digest of the shipped library: per kernel, how many wgmma / TMA / mbarrier SASS instructions it holds
+(cuobjdump -sass), plus the proof of absence of the legacy mma.sync tensor-core path (HMMA / IMMA).  Written to
 profiles/<tag>_sass_digest.txt; runs on the build host (no GPU needed).
 
   python scripts/sass_digest.py [tag]
@@ -12,8 +12,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "omg_b200", "lib", "libomg_b200.so")
-WATCH = ("UTCHMMA", "UTCQMMA", "UTCBAR", "UTCCP", "UTCATOMSWS", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTMAPF", "UTMACCTL",
-         "SYNCS", "HMMA", "IMMA", "WGMMA", "QGMMA", "MUFU.EX2", "FFMA2", "FADD2", "FMUL2", "LDGSTS", "BAR.SYNC", "ERRBAR")
+WATCH = ("HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "UTMACCTL", "SYNCS", "USETMAXREG", "HMMA", "IMMA",
+         "MUFU.EX2", "LDGSTS", "BAR.SYNC", "ERRBAR")
 
 
 def main():
@@ -34,18 +34,15 @@ def main():
             per[cur]["_total"] += 1
             for w in WATCH:
                 if op.startswith(w):
-                    key = w
-                    if w == "UTCHMMA" and ".2CTA" in op:
-                        key = "UTCHMMA.2CTA"
-                    per[cur][key] += 1
-    out = [f"# SASS opcode digest of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass, sm_100a)", ""]
+                    per[cur][w] += 1
+    out = [f"# SASS opcode digest of {os.path.relpath(LIB, ROOT)} (cuobjdump -sass, sm_90a)", ""]
     tot = collections.Counter()
     for fn, c in per.items():
         tot.update(c)
         cols = "  ".join(f"{k}={v}" for k, v in sorted(c.items()) if k != "_total")
         out.append(f"{fn}\n    instructions={c['_total']}  {cols}")
     out += ["", "TOTAL  " + "  ".join(f"{k}={v}" for k, v in sorted(tot.items()) if k != "_total"),
-            f"legacy tensor-core opcodes: HMMA={tot['HMMA']} IMMA={tot['IMMA']} WGMMA={tot['WGMMA']}"]
+            f"legacy tensor-core opcodes: HMMA={tot['HMMA']} IMMA={tot['IMMA']}"]
     path = os.path.join(ROOT, "profiles", f"{tag}_sass_digest.txt")
     open(path, "w").write("\n".join(out) + "\n")
     print("\n".join(out[-2:]))

@@ -1,7 +1,7 @@
 """BASELINE config 1 at FULL SDXL widths (2.57 G parameters): one fusion step of stage 2 (step index 16) at 64x64
 latents, main UNet rows (B=4, prompt-to-prompt self-replace window active) + one LoRA concept (B=2) as ONE grouped
 forward, then omg_fuse_step; compared with the fp32 oracle on the host cores.  Tolerances (1.25 x measured): 2.2e-3 / 2.9e-3 on the noise
-prediction, 3e-3 on the latents after the step (measured: 1.7e-3 / 2.3e-3 / 1.1e-3)."""
+prediction, 3e-3 on the latents after the step."""
 import os
 import time
 

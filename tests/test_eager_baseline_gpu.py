@@ -1,6 +1,6 @@
 """The number to beat on the same GPU (SURVEY 8d, CPU-baseline row): the reference's actual library path - torch eager
 fp16 (cuBLAS / cuDNN), probabilities materialised for the prompt-to-prompt controller - restated by the oracle and run
-on the B200, timed for one main-UNet call (B=4, 128x128 latents) next to the CUDA path's graph replay.  Test
+on the same GPU, timed for one main-UNet call (B=4, 128x128 latents) next to the CUDA path's graph replay.  Test
 infrastructure: the only assertion is that the hand-written path is faster."""
 import time
 

@@ -155,7 +155,7 @@ def test_self_attention(ops, B, N, heads):
 
 
 @pytest.mark.parametrize("n_q,n_kv,gain", [(256, 200, 1.0), (130, 321, 1.0), (512, 640, 2.5), (128, 129, 2.5),
-                                            (384, 1024, 3.0)])
+                                            (384, 1024, 3.0), (121, 121, 1.0), (200, 57, 1.0), (64, 63, 2.5)])
 def test_attention_block_edges(ops, n_q, n_kv, gain):
     """Self-attention kernel edges: odd block counts, a partial last block, n_q != n_kv, and score ranges large enough
     that the lazy O rescale fires; with and without `accumulate`."""
@@ -176,7 +176,8 @@ def test_attention_block_edges(ops, n_q, n_kv, gain):
 
 
 @pytest.mark.parametrize("B,n_q,n_kv,heads", [(4, 1024, 77, 20), (2, 4096, 77, 10), (2, 200, 16, 3), (1, 128, 128, 7),
-                                              (2, 300, 100, 5), (1, 64, 5, 1), (8, 1024, 77, 20)])
+                                              (2, 300, 100, 5), (1, 64, 5, 1), (8, 1024, 77, 20), (2, 256, 57, 3),
+                                              (1, 130, 121, 2), (1, 100, 59, 1)])
 def test_cross_attention_head_group_kernel(ops, B, n_q, n_kv, heads):
     """Cross-attention kernel (one key block, a CTA walks a group of heads): text keys (77), IP tokens (16), padded key
     counts, ragged query tiles, head counts with a tail group; remapped rows and the accumulate / out_weight term."""
@@ -340,43 +341,6 @@ def test_layernorm_folded_into_gemm_pair(ops, M, C, N, geglu):
     assert rel(out, y) < 3e-3
 
 
-@pytest.mark.parametrize("M,N,K", [(4096, 3840, 1280), (2176, 512, 256), (256, 256, 64), (8192, 1280, 640), (300, 768, 320)])
-def test_linear_cta_pair(ops, M, N, K):
-    """cta_group::2: a CTA pair computes 256 x 256 tiles (odd m-tile counts and ragged M included)."""
-    x, w, b = rnd(M, K, seed=1), rnd(N, K, scale=K ** -0.5, seed=2), rnd(N, seed=3)
-    r = rnd(M, N, seed=4)
-    ref = x.float() @ w.float().t() + b.float() + r.float()
-    for bn in (256, 160):
-        out = ops.linear(x, w, bias=b, residual=r, block_n=bn, cta_pair=2)
-        assert rel(out, ref) < 2e-3
-        out1 = ops.linear(x, w, bias=b, residual=r, block_n=bn, cta_pair=1)
-        assert torch.equal(out, out1)  # same accumulation order per element: bit-identical to single-CTA tiles
-
-
-def test_cta_pair_geglu_lora_conv(ops):
-    M, C = 2048, 640
-    x = rnd(M, C, seed=1)
-    w, b = rnd(8 * C, C, scale=C ** -0.5, seed=2), rnd(8 * C, seed=3)
-    wi, bi = ops.pack_geglu_weight(w, b)
-    out = ops.linear(x, wi, bias=bi, epilogue=1, cta_pair=2)
-    h = x.float() @ w.float().t() + b.float()
-    assert rel(out, h[:, :4 * C] * F.gelu(h[:, 4 * C:])) < 2e-3
-    # LoRA second weight matrix through the pair path
-    N, R = 1280, 64
-    wq, a, bw = rnd(N, C, scale=C ** -0.5, seed=4), rnd(R, C, scale=C ** -0.5, seed=5), rnd(N, R, scale=0.05, seed=6)
-    t = ops.linear(x, a)
-    out = ops.linear(x, wq, lora=(t, bw), block_n=256, cta_pair=2)
-    assert rel(out, x.float() @ wq.float().t() + t.float() @ bw.float().t()) < 2e-3
-    # conv3x3 with time-embedding row vector
-    B, H, W, Cin, Nc = 2, 32, 32, 128, 512
-    xi = rnd(B, H, W, Cin, seed=7)
-    wc = rnd(Nc, Cin, 3, 3, scale=(9 * Cin) ** -0.5, seed=8)
-    bc, temb = rnd(Nc, seed=9), rnd(B, Nc, seed=10)
-    out = ops.conv3x3(xi, ops.pack_conv3x3_weight(wc), bias=bc, rowvec=temb, block_n=256, cta_pair=2)
-    ref = F.conv2d(xi.float().permute(0, 3, 1, 2), wc.float(), bc.float(), padding=1) + temb.float()[:, :, None, None]
-    assert rel(out.permute(0, 3, 1, 2), ref) < 2e-3
-
-
 @pytest.mark.parametrize("M,N,K", [(4096, 1280, 1280), (2176, 640, 512), (384, 320, 128), (8192, 1280, 5120)])
 def test_linear_tall_tiles(ops, M, N, K):
     """256 x 160 tiles in one CTA (two 128-row sub-tiles share each weight tile); odd m-tile counts included."""
@@ -503,7 +467,7 @@ def test_column_statistics_of_down_and_up_convs(ops):
 
 
 def test_pair320_tiles_conv_residual_stats_and_lora(ops):
-    """256 x 320 CTA-pair tiles (two N = 160 MMAs per K step, one 320-column accumulator): a conv with time-embedding
+    """128 x 320 tiles (two N = 160 wgmmas per K step, one 320-column accumulator): a conv with time-embedding
     row vector and residual, GroupNorm column statistics and LayerNorm row statistics out of the same epilogue, an
     un-merged LoRA K-segment against the second weight matrix."""
     from omg_b200 import _lib as L
@@ -517,7 +481,7 @@ def test_pair320_tiles_conv_residual_stats_and_lora(ops):
         + res.float().permute(0, 3, 1, 2)
     assert rel(out.permute(0, 3, 1, 2), ref) < 2e-3
     assert torch.allclose(part.sum(1)[..., 0], out.float().sum((1, 2)), rtol=1e-3, atol=5e-2)
-    # row statistics (LayerNorm fold producer) + LoRA segment, default tile choice (auto-upgraded from 160 to 320)
+    # row statistics (LayerNorm fold producer) + LoRA segment, default tile choice
     M, C = 1024, 640
     o, wo = rnd(M, C, seed=6), rnd(C, C, scale=C ** -0.5, seed=7)
     t, b2 = rnd(M, 32, seed=8), rnd(C, 32, scale=0.1, seed=9)

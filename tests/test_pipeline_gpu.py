@@ -1,7 +1,7 @@
 """GPU parity of the full two-stage loops (LoRA and InstantID variants) against oracle.pipeline.denoise on the tiny
 topology: 18 steps so that the fusion window (step index > 15) is exercised, P2P self-replace threshold 8x8 tokens,
-two concepts with disjoint masks.  Final-latent tolerances = 1.3 x the values measured on a B200 (LoRA 2.11e-3, style / None-mask 1.69e-3,
-InstantID 1.00e-3: 18 chained UNet calls at fp16 storage vs the fp32 oracle)."""
+two concepts with disjoint masks.  Final-latent tolerances allow for 18 chained UNet calls at fp16 storage vs the fp32
+oracle."""
 import os
 
 import pytest
@@ -136,6 +136,7 @@ def test_instantid_two_stage_pipeline(share):
     idsd = weights(cfg, 41, controlnet=True)
     size = 128
     rs = torch.load(os.path.join(G, "resampler.pt"))
+    rs["sd"] = {k: v.float() for k, v in rs["sd"].items()}  # stored as fp16 (fp16-representable values)
     ipw = {k: (r16(a), r16(b)) for k, (a, b) in synthetic.make_ip_adapter(cfg, 31).items()}
     pipe = InstantidMultiConceptPipeline(PackedUNet(cfg, sd), controlnet=PackedUNet(cfg, idsd, controlnet=True))
     prompts = ["two people"] * 2
@@ -303,7 +304,7 @@ def test_main_pass_controlnet_condition_change_with_graphs():
                       controlnet_scale=0.7)
         e = rel(outs[k], ref)
         print("main-pass controlnet pipeline rel err", e)
-        assert e < 3.5e-3   # measured 2.7e-3: 4 large Euler steps at guidance 5 (main UNet + ControlNet per step)
+        assert e < 3.5e-3   # measured on H100: 2.5e-3 / 2.6e-3: 4 large Euler steps at guidance 5 (main UNet + ControlNet per step)
 
 
 def test_instantid_main_pass_controlnet_together_with_identitynet():
@@ -321,6 +322,7 @@ def test_instantid_main_pass_controlnet_together_with_identitynet():
     sd, idsd, c2sd = weights(cfg, 0), weights(cfg, 41, controlnet=True), weights(cfg, 42, controlnet=True)
     size = 128
     rs = torch.load(os.path.join(G, "resampler.pt"))
+    rs["sd"] = {k: v.float() for k, v in rs["sd"].items()}  # stored as fp16 (fp16-representable values)
     ipw = {k: (r16(a), r16(b)) for k, (a, b) in synthetic.make_ip_adapter(cfg, 31).items()}
     pipe = InstantidMultiConceptPipeline(PackedUNet(cfg, sd), controlnet=PackedUNet(cfg, idsd, controlnet=True))
     pipe.controlnet2 = PackedUNet(cfg, c2sd, controlnet=True)
@@ -352,4 +354,4 @@ def test_instantid_main_pass_controlnet_together_with_identitynet():
                   identitynet=ou.Ctx(idsd, ocfg(cfg)), identity_cond=kps[None].repeat(2, 1, 1, 1), identity_scale=0.8)
     e = rel(out, ref)
     print("instantid + main-pass controlnet pipeline rel err", e)
-    assert e < 1.3e-3   # measured 0.96e-3
+    assert e < 1.3e-3   # measured on H100: 0.96e-3

@@ -3,6 +3,7 @@ stages) executed on this repo's kernels, against golden vectors produced by the 
 (tests/golden/make_golden.py imports src/efficientvit: LiteMLA, EfficientViTBlock, EfficientViTLargeBackbone, SamNeck,
 EfficientViTSamImageEncoder) - this row's oracle is the reference itself.  Plus the four non-GEMM kernels against torch."""
 import os
+import sys
 
 import pytest
 import torch
@@ -10,6 +11,8 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(__file__), "golden", "sam_encoder.pt")
+sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
+from make_golden import sam_input  # noqa: E402  (pure helper; does not import the reference)
 
 
 def rel(a, b):
@@ -82,27 +85,28 @@ def test_lite_mla_and_efficientvit_block_match_the_reference_modules():
     from omg_b200.sam_encoder import efficientvit_block, lite_mla
     d = torch.load(G)
     to = lambda t: t.permute(0, 2, 3, 1).contiguous().cuda()  # noqa: E731
-    y = lite_mla({"m." + k: v for k, v in d["mla_sd"].items()}, "m", to(d["mla_x"]))
+    y = lite_mla({"m." + k: v for k, v in d["mla_sd"].items()}, "m", to(sam_input("mla").half()))
     e1 = rel(y.permute(0, 3, 1, 2), d["mla_y"])
-    y = efficientvit_block({"b." + k: v for k, v in d["blk_sd"].items()}, "b", to(d["blk_x"]))
+    y = efficientvit_block({"b." + k: v for k, v in d["blk_sd"].items()}, "b", to(sam_input("blk").half()))
     e2 = rel(y.permute(0, 3, 1, 2), d["blk_y"])
     print("LiteMLA rel err", e1, "EfficientViTBlock rel err", e2)
-    assert e1 < 5e-4 and e2 < 5e-4   # measured 3.6e-4 / 3.6e-4
+    assert e1 < 5e-4 and e2 < 5e-4   # measured on H100: 3.9e-4 / 3.5e-4
 
 
 def test_sam_image_encoder_matches_the_reference_module():
     from omg_b200.sam_encoder import PackedSamImageEncoder
     d = torch.load(G)
     enc = PackedSamImageEncoder(d["sd"], device="cuda")
-    y, feats = enc(d["x"], return_features=True)
-    assert tuple(y.shape) == tuple(d["y"].shape) == (1, 256, 64, 64)
+    x = sam_input().half()
+    y, feats = enc(x, return_features=True)
+    assert tuple(y.shape) == (1, 256, 64, 64)
     assert {f"stage{k}": tuple(v.shape) for k, v in feats.items()} == {k: v for k, v in d["stage_shapes"].items()
                                                                          if k.startswith("stage") and k != "stage_final"}
-    e3, e5, e = rel(feats[3], d["stage3"]), rel(feats[5], d["stage5"]), rel(y, d["y"])
+    e3, e5, e = rel(feats[3], d["stage3"]), rel(feats[5], d["stage5"]), rel(y[..., ::8, ::8], d["y_sub"])
     print("sam encoder rel err: stage3", e3, "stage5", e5, "output", e)
-    assert e3 < 5.5e-4 and e5 < 6e-4 and e < 8.5e-4   # measured 4.1e-4 / 4.5e-4 / 6.5e-4
+    assert e3 < 5.5e-4 and e5 < 6e-4 and e < 8.5e-4   # measured on H100: 4.6e-4 / 4.6e-4 / 6.4e-4
     # the call above captured a CUDA graph; a replay on another image must equal the eager launches for that image bit for bit
-    x2 = d["x"].flip(-1) * 0.5
+    x2 = x.flip(-1) * 0.5
     y2 = enc(x2, return_features=True)[0]
     eager = PackedSamImageEncoder(d["sd"], device="cuda", use_graph=False)
-    assert torch.equal(y2, eager(x2)) and torch.equal(enc(d["x"], return_features=True)[0], y) and not torch.equal(y2, y)
+    assert torch.equal(y2, eager(x2)) and torch.equal(enc(x, return_features=True)[0], y) and not torch.equal(y2, y)

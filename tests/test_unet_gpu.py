@@ -1,6 +1,6 @@
 """GPU parity of the UNet / ControlNet executor and of both pipelines against the fp32 CPU oracle, tiny topology
 (same code paths as SDXL: conv tails, GroupNorm over concatenated skips, P2P remaps, LoRA K-segments, IP-adapter,
-ControlNet residuals).  Tolerance: relative L2 <= 1.9e-3 per UNet call = 1.25 x the largest value measured on a B200 (1.50e-3, general
+ControlNet residuals).  Tolerance: relative L2 <= 1.9e-3 per UNet call (the largest error is the general
 P2P two-term step; fp16 storage vs the fp32 oracle fed the same fp16-rounded weights)."""
 import pytest
 import torch
@@ -49,8 +49,8 @@ def test_plain_unet(env):
 
 def test_fp32_trunk_twins(env):
     """Opt-in fp32 master copy of the residual trunk (UNetRunner.trunk_f32): the residual GEMMs read / write fp32 twins.
-    Same bound as the default path on the tiny topology (the gain shows at SDXL depth: config 2 final latents 1.53e-3 ->
-    1.17e-3, profiles/r02_parity_fullwidth_trunk_f32.jsonl), and the twins are really used (results differ bitwise)."""
+    Same bound as the default path on the tiny topology (the gain shows at SDXL depth, over many chained residual adds),
+    and the twins are really used (results differ bitwise)."""
     from omg_b200.unet import UNetRunner
     from oracle import unet as ou
     cfg = env["cfg"]
