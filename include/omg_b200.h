@@ -37,7 +37,8 @@ typedef struct {
     int32_t b_idx; /* 0: columns of w, 1: columns of w2 (e.g. the LoRA up-projection B, kept un-merged) */
 } omg_seg;
 
-enum { OMG_EPI_NONE = 0, OMG_EPI_GEGLU = 1, OMG_EPI_SILU = 2, OMG_EPI_QUICK_GELU = 3, OMG_EPI_GELU = 4, OMG_EPI_GELU_TANH = 5 };
+enum { OMG_EPI_NONE = 0, OMG_EPI_GEGLU = 1, OMG_EPI_SILU = 2, OMG_EPI_QUICK_GELU = 3, OMG_EPI_GELU = 4, OMG_EPI_GELU_TANH = 5,
+       OMG_EPI_RELU = 6 };
 
 /*
  * out[pix, n] = epi( sum_seg sum_k A_seg[pix+(dx,dy), k] * W[n, b_k0+k] + bias[n] + rowvec[b, n] ) + residual[pix, n]
@@ -48,7 +49,8 @@ enum { OMG_EPI_NONE = 0, OMG_EPI_GEGLU = 1, OMG_EPI_SILU = 2, OMG_EPI_QUICK_GELU
  * OMG_EPI_GEGLU: W rows (and bias) are interleaved (value_j, gate_j) pairs; out has N/2 channels,
  * out_j = value_j * gelu_erf(gate_j).   OMG_EPI_SILU: epi(x) = x * sigmoid(x) (time-embedding MLPs).
  * OMG_EPI_QUICK_GELU: x * sigmoid(1.702 x), OMG_EPI_GELU: erf-gelu (the fc1 activations of the two CLIP text towers,
- * transformers CLIPMLP [3P], reached from src/pipelines/lora_pipeline.py:315-347).
+ * transformers CLIPMLP [3P], reached from src/pipelines/lora_pipeline.py:315-347).  OMG_EPI_RELU: max(x, 0) (the MLP,
+ * hypernetwork and IoU-head layers of the SAM mask decoder, segment_anything MaskDecoder / TwoWayTransformer [3P]).
  */
 typedef struct {
     omg_view4 a[OMG_MAX_A];
@@ -236,6 +238,39 @@ int omg_dwconv(const void* x, const void* w, const void* bias, void* y, int B, i
 int omg_group1x1(const void* x, const void* w, void* y, long long pixels, int C, int ldx, int ldy, int group, void* stream);
 int omg_relu_linear_attention(const void* qkv, void* out, int B, int N, int heads, int dim, float eps, void* stream);
 int omg_resize_bicubic(const void* x, void* y, int B, int H, int W, int C, int Ho, int Wo, void* stream);
+
+/*
+ * EfficientViT-SAM prompt-to-mask path (SURVEY 8f-4): segment_anything's MaskDecoder / TwoWayTransformer [3P] as the
+ * reference builds them (src/efficientvit/models/efficientvit/sam.py:520-544) and EfficientViTSam.postprocess_masks
+ * (sam.py:224-241).  Projections, MLPs, hypernetworks and the IoU head run on omg_gemm, LayerNorm on omg_layernorm.
+ *
+ * omg_attention_small: softmax(scale Q K^T) V per head for head_dim 16 | 32 when one side is short, fp32 softmax.  The
+ *   descriptor is omg_attn_desc (items remap batches; out_weight must be 1, accumulate and causal 0; q / out rows 16 B
+ *   aligned).  n_kv <= 64 (image -> token, token self-attention): K/V of the item and head live in shared memory, any
+ *   n_q.  Otherwise n_q <= 64 (token -> image): the keys are split over CTAs of 128, and `ws` must hold
+ *   OMG_ATTN_SMALL_WS_FLOATS(n_items, heads, n_q, n_kv) floats for the (acc, max, sum) partials that a second launch
+ *   combines.
+ */
+#define OMG_ATTN_SMALL_WS_FLOATS(items, heads, n_q, n_kv) \
+    ((long long)(items) * (heads) * (n_q) * (((n_kv) + 127) / 128) * 36)
+int omg_attention_small(const omg_attn_desc* desc, void* ws, void* stream);
+
+/*
+ * omg_sam_mask_head: MaskDecoder.output_upscaling after its first ConvTranspose2d, fused with the hypernetwork product:
+ *   out[b, m, 2Y+ey, 2X+ex] = sum_o hyper[b, m, o] gelu(b2[o] + sum_c gelu(LN2d(up1[b, Y, X, :]))[c] w2[ey, ex, c, o])
+ * up1: fp16 [B, 64, 64, 2, 2, 64] = ConvTranspose2d(256 -> 64, k2, s2) as omg_gemm writes it with weight rows
+ * (dy, dx, channel): element (b, 2y + dy, 2x + dx, c) of the 128 x 128 map.  ln_w / ln_b fp32 [64] (LayerNorm2d, eps);
+ * w2 fp32 [2][2][64][32] (ConvTranspose2d(64 -> 32) weight [c, o, ey, ex] permuted), b2 fp32 [32]; hyper fp16,
+ * element (b, m, o) at hyper + b * hyper_bs + m * hyper_ms + o; M <= 4 masks.  out fp32 [B, M, 256, 256] low-res logits.
+ *
+ * omg_sam_postprocess: bilinear (align_corners = False) low x low -> mid x mid, crop to [h_in, w_in], bilinear -> H x W,
+ * evaluated as one composite per output pixel of lowres fp32 [BM, low, low].  mask (uint8 / bool [BM, H, W]) gets
+ * value > threshold, logits (fp32 [BM, H, W]) the value; either may be NULL.
+ */
+int omg_sam_mask_head(const void* up1, const void* ln_w, const void* ln_b, const void* w2, const void* b2, const void* hyper,
+                      long long hyper_bs, long long hyper_ms, int B, int M, float eps, void* out, void* stream);
+int omg_sam_postprocess(const void* lowres, int BM, int low, int mid, int h_in, int w_in, int H, int W, float threshold,
+                        void* mask, void* logits, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Launch plans: a forward as a handle.  The reference drives one UNet forward as a Python call

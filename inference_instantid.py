@@ -2,13 +2,15 @@
 """OMG + InstantID multi-identity generation on the H100 path.  The reference CLI's flags (names, defaults, types:
 inference_instantid.py:259-286, pinned by tests/golden/cli_flags.json), prompt mini-DSL, two-stage flow and output
 files; additions (non-breaking): --synthetic, --tiny, --num_inference_steps, --image_size, --dedup, --mask_boxes,
---face_embeds, --face_kps.
+--face_embeds, --face_kps, --sam_boxes.
 
 Face analysis (insightface antelopev2), segmentation and the VAE sit outside the accelerated hot path (SURVEY section
 8): when `insightface` is not importable the identities come from --face_embeds (one 512-d .pt / .npy per region) and
 the stage-2 key-points from --face_kps; regions come from --mask_boxes.  In --synthetic mode identities are unit-norm
 random 512-d embeddings (seeds 1, 2), the IdentityNet condition is the reference's `draw_kps_multi` rendering of fixed
-key-points and the masks are the config rectangles.
+key-points and the masks are the config rectangles.  --sam_boxes (EfficientViT-SAM masks from box prompts, see
+inference_lora.py) needs a decoded stage-1 image; this CLI keeps its stage-1 output as latents, so the flag is checked
+against --mask_boxes and then refused with that reason.
 """
 import argparse
 import math
@@ -94,6 +96,8 @@ def parse_args():
     p.add_argument("--num_inference_steps", default=50, type=int)
     p.add_argument("--image_size", default=1024, type=int)
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
+    p.add_argument("--sam_boxes", default="", type=str, help="x0,y0,x1,y1|... box prompts for EfficientViT-SAM on the "
+                   "decoded stage-1 image (needs a decoded image; excludes --mask_boxes)")
     p.add_argument("--face_embeds", default="", type=str, help="a.pt|b.pt: 512-d identity embeddings, one per region "
                    "(replaces insightface on the reference images)")
     p.add_argument("--face_kps", default="", type=str, help="JSON file: list of five (x, y) key-points per face for "
@@ -243,6 +247,8 @@ if __name__ == "__main__":
             masks.append(m)
         masks = masks or [None] * len(regions)
     pipe.dedup = args.dedup
+    from omg_b200.sam import check_sam_flags
+    check_sam_flags(args.sam_boxes, args.mask_boxes, decoded=getattr(pipe, "vae_decoder", None) is not None)
     input_prompt = [prompts, regions]
     common = dict(input_prompt=input_prompt, concept_models=cm, input_neg_prompt=[args.negative_prompt] * len(input_prompt),
                   controller=controller, face_app=face_app, controlnet_conditioning_scale=args.IdentityNet_rate,

@@ -1,12 +1,15 @@
 #!/usr/bin/env python
 """OMG + LoRA multi-concept generation on the H100 path.  Same flags, prompt mini-DSL, two-stage flow and output
 files as the reference CLI (inference_lora.py:201-323); additions (non-breaking): --synthetic, --num_inference_steps,
---image_size, --mask_boxes, --vae_fp16_safe.
+--image_size, --mask_boxes, --vae_fp16_safe, --sam_boxes.
 
-The segmentation models between the stages (YOLO-World / GroundingDINO + SAM) and the VAE / text encoders are outside
-the accelerated hot path (SURVEY section 8): masks come from --mask_boxes (x0,y0,x1,y1 per concept, '|' separated) or,
-in --synthetic mode, from the fixed config-2 rectangles; without a VAE the latents are saved (stage-{1,2}.pt) next to
-a PNG visualisation of their first three channels.
+Masks between the stages: with --sam_boxes (x0,y0,x1,y1 per concept, '|' separated, stage-1 pixels) the boxes prompt
+EfficientViT-SAM xl1 on the decoded stage-1 image, as the reference's predict_mask does with a detector's box
+(inference_lora.py:91-126), and the device masks go straight into stage 2 (weights from --efficientViT_checkpoint, or
+random with --synthetic; needs a decoded image: --vae_fp16_safe or --synthetic --decode).  The detectors (YOLO-World /
+GroundingDINO) stay outside: boxes are an input.  --mask_boxes instead fills the boxes as rectangles; in --synthetic mode
+without either flag the masks are the fixed config-2 rectangles.  Without a VAE the latents are saved (stage-{1,2}.pt)
+next to a PNG visualisation of their first three channels.
 """
 import argparse
 import hashlib
@@ -74,6 +77,9 @@ def parse_args():
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
     p.add_argument("--vae_fp16_safe", default="", type=str, help="directory of fp16-safe SDXL VAE weights: decode to "
                    "PNG on the GPU (without it the latents are saved)")
+    p.add_argument("--sam_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (stage-1 pixels, one per concept, "
+                   "empty = skip the concept): box prompts for EfficientViT-SAM on the decoded stage-1 image, whose masks "
+                   "drive stage 2; needs a decoded image, excludes --mask_boxes")
     return p.parse_args()
 
 
@@ -166,6 +172,16 @@ if __name__ == "__main__":
         vcfg = VaeConfig.tiny() if args.tiny else VaeConfig.sdxl()
         pipe.vae_decoder = PackedVaeDecoder(synthetic.make_vae_state_dict(vcfg, 0), vcfg, device=device)
     decoded = pipe.vae_decoder is not None
+    from omg_b200 import sam as sam_lib
+    sam_lib.check_sam_flags(args.sam_boxes, args.mask_boxes, decoded)
+    sam_boxes = None
+    if args.sam_boxes:
+        try:
+            sam_boxes = sam_lib.parse_sam_boxes(args.sam_boxes)
+        except ValueError as e:
+            raise SystemExit(str(e))
+        if len(sam_boxes) != len(pipe_list):
+            raise SystemExit(f"--sam_boxes has {len(sam_boxes)} entries for {len(pipe_list)} concepts")
     if decoded:
         kwargs["output_type"] = "pil"  # lora_pipeline.py:634-661: VAE decode + postprocess
     styleL = bool(args.style_lora) and os.path.exists(args.style_lora)
@@ -182,6 +198,17 @@ if __name__ == "__main__":
             m = torch.zeros(height, width)
             m[y0:y1, x0:x1] = 1
             masks.append(m)
+    elif sam_boxes is not None:
+        # predict_mask (inference_lora.py:91-126) with the boxes as the detections: EfficientViT-SAM on the decoded
+        # stage-1 image, masks stay on the device
+        if args.synthetic:
+            from omg_b200 import synthetic
+            sam_model = sam_lib.create_sam_model("xl1", state_dict=synthetic.make_sam_state_dict(0))
+        else:
+            sam_model = sam_lib.create_sam_model("xl1", weight_url=args.efficientViT_checkpoint)
+        masks = sam_lib.sam_region_masks(sam_lib.EfficientViTSamPredictor(sam_model), image[0], sam_boxes)
+        for k, m in enumerate(masks):
+            print(f"SAM mask {k}: " + ("no box, concept skipped" if m is None else f"{int(m.sum())} pixels"))
     else:
         masks = synth_masks
     if any(m is not None for m in masks):

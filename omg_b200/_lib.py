@@ -10,7 +10,7 @@ OMG_MAX_A = 4
 OMG_MAX_SEGS = 12
 OMG_ATTN_MAX_ITEMS = 16
 OMG_MAX_CONCEPTS = 8
-EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_QUICK_GELU, EPI_GELU, EPI_GELU_TANH = 0, 1, 2, 3, 4, 5
+EPI_NONE, EPI_GEGLU, EPI_SILU, EPI_QUICK_GELU, EPI_GELU, EPI_GELU_TANH, EPI_RELU = 0, 1, 2, 3, 4, 5, 6
 
 
 class View4(C.Structure):
@@ -79,6 +79,11 @@ SYMBOLS = {
     "omg_group1x1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "omg_relu_linear_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "omg_resize_bicubic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "omg_attention_small": (C.c_int, [C.POINTER(AttnDesc), C.c_void_p, C.c_void_p]),
+    "omg_sam_mask_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
+                                    C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
+    "omg_sam_postprocess": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
     "omg_plan_create": (C.c_void_p, []),
     "omg_plan_destroy": (None, [C.c_void_p]),
     "omg_plan_record_begin": (C.c_int, [C.c_void_p]),

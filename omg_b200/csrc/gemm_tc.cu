@@ -354,6 +354,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                                 } else if (p.act_silu == 4) {  // tanh-gelu (EfficientViT-SAM): 0.5 x (1 + tanh(sqrt(2/pi)(x + 0.044715 x^3)))
                                     const float u = 0.7978845608028654f * fmaf(0.044715f * v * v, v, v);
                                     v = 0.5f * v * (2.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * u)));
+                                } else if (p.act_silu == 5) {  // ReLU (SAM mask decoder MLPs)
+                                    v = fmaxf(v, 0.f);
                                 }
                                 x[h][e] = v;
                             }
@@ -558,7 +560,8 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     OMG_CHECK(d->Ktot % 8 == 0, "omg_gemm: Ktot=%d must be a multiple of 8", d->Ktot);
     const bool geglu = d->epilogue == OMG_EPI_GEGLU;
     const bool silu = d->epilogue == OMG_EPI_SILU;
-    const int act = silu ? 1 : (d->epilogue == OMG_EPI_QUICK_GELU ? 2 : (d->epilogue == OMG_EPI_GELU ? 3 : (d->epilogue == OMG_EPI_GELU_TANH ? 4 : 0)));
+    const int act = silu ? 1 : (d->epilogue == OMG_EPI_QUICK_GELU ? 2 : (d->epilogue == OMG_EPI_GELU ? 3 : (d->epilogue == OMG_EPI_GELU_TANH ? 4 :
+                    (d->epilogue == OMG_EPI_RELU ? 5 : 0))));
     OMG_CHECK(d->epilogue == OMG_EPI_NONE || geglu || act, "omg_gemm: unknown epilogue %d", d->epilogue);
     const int N_out = geglu ? d->N / 2 : d->N;
     OMG_CHECK(d->d.C == N_out, "omg_gemm: output view has %d channels, expected %d", d->d.C, N_out);
@@ -601,7 +604,7 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     p.rowvec_ld = d->rowvec_ld;
     p.residual = static_cast<const __half*>(d->residual);
     p.residual_ld = d->residual_ld;
-    p.act_silu = act;  // 0 none, 1 SiLU, 2 quick_gelu, 3 erf-gelu, 4 tanh-gelu
+    p.act_silu = act;  // 0 none, 1 SiLU, 2 quick_gelu, 3 erf-gelu, 4 tanh-gelu, 5 ReLU
     p.stats_out = static_cast<float*>(d->row_stats_out);
     p.stats_in = static_cast<const float*>(d->row_stats_in);
     p.stats_parts = d->row_stats_parts;

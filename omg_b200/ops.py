@@ -246,6 +246,74 @@ def attention(q, k, v, out, heads, n_q, n_kv, items, q_col0=0, k_col0=0, v_col0=
     return out
 
 
+def attention_small_ws(n_items, heads, n_q, n_kv, device="cuda"):
+    """fp32 workspace of the split-key path of attention_small (OMG_ATTN_SMALL_WS_FLOATS)."""
+    n = min(n_items, L.OMG_ATTN_MAX_ITEMS) * heads * n_q * ((n_kv + 127) // 128) * 36
+    return torch.empty(n, dtype=torch.float32, device=device)
+
+
+def attention_small(q, k, v, out, heads, head_dim, n_q, n_kv, q_col0=0, k_col0=0, v_col0=0, out_col0=0, scale=None,
+                    ws=None, items=None):
+    """softmax(scale Q K^T) V per head for head_dim 16 | 32 with one short side (<= 64 tokens): q/k/v/out are
+    [batch, tokens, ld] fp16 column views (a head's columns at col0 + head_dim * h).  items: list of (out_b, q_b, k_b, v_b),
+    default one per batch; more than 16 items are issued as several launches.  ws: attention_small_ws(...) when
+    n_kv > 64 (the split-key path)."""
+    for t in (q, k, v, out):
+        _chk16(t)
+        assert t.dim() == 3 and t.stride(2) == 1
+    if items is None:
+        items = [(b, b, b, b) for b in range(out.shape[0])]
+    if n_kv > 64 and ws is None:
+        ws = attention_small_ws(len(items), heads, n_q, n_kv, q.device)
+    for i0 in range(0, len(items), L.OMG_ATTN_MAX_ITEMS):
+        chunk = items[i0:i0 + L.OMG_ATTN_MAX_ITEMS]
+        d = L.AttnDesc()
+        d.q, d.q_ld, d.q_bs, d.q_col0 = q.data_ptr(), q.stride(1), q.stride(0), q_col0
+        d.k, d.k_ld, d.k_bs, d.k_col0 = k.data_ptr(), k.stride(1), k.stride(0), k_col0
+        d.v, d.v_ld, d.v_bs, d.v_col0 = v.data_ptr(), v.stride(1), v.stride(0), v_col0
+        d.out, d.out_ld, d.out_bs, d.out_col0 = out.data_ptr(), out.stride(1), out.stride(0), out_col0
+        d.n_q, d.n_kv, d.heads, d.head_dim = n_q, n_kv, heads, head_dim
+        d.n_items = len(chunk)
+        for i, (ob, qb, kb, vb) in enumerate(chunk):
+            d.out_b[i], d.q_b[i], d.k_b[i], d.v_b[i] = ob, qb, kb, vb
+        d.scale = head_dim ** -0.5 if scale is None else scale
+        d.out_weight, d.accumulate, d.causal = 1.0, 0, 0
+        L.check(L.load().omg_attention_small(C.byref(d), _ptr(ws), _stream()), "omg_attention_small")
+    return out
+
+
+def sam_mask_head(up1, ln_w, ln_b, w2, b2, hyper, M, eps=1e-6, out=None):
+    """SAM output_upscaling after ConvTranspose2d #1 + hypernetwork product (omg_sam_mask_head).  up1 fp16
+    [B, 64, 64, 2, 2, 64] (or [B*4096, 256]); w2 fp32 [2, 2, 64, 32]; hyper fp16 (B, M, 32) view with unit channel
+    stride -> fp32 (B, M, 256, 256) low-res logits."""
+    _chk16(up1)
+    _chk16(hyper)
+    assert up1.is_contiguous() and hyper.stride(-1) == 1
+    B = up1.numel() // (4096 * 256)
+    if out is None:
+        out = torch.empty((B, M, 256, 256), dtype=torch.float32, device=up1.device)
+    L.check(L.load().omg_sam_mask_head(up1.data_ptr(), ln_w.data_ptr(), ln_b.data_ptr(), w2.data_ptr(), b2.data_ptr(),
+                                       hyper.data_ptr(), hyper.stride(0), hyper.stride(1), B, M, float(eps), out.data_ptr(),
+                                       _stream()), "omg_sam_mask_head")
+    return out
+
+
+def sam_postprocess(lowres, input_size, original_size, mid=1024, threshold=0.0, mask=None, logits=None,
+                    return_mask=True, return_logits=False):
+    """postprocess_masks + threshold (omg_sam_postprocess): lowres fp32 (B, M, low, low) -> (bool mask, fp32 logits)
+    at original_size (either None when not requested)."""
+    assert lowres.is_cuda and lowres.dtype == torch.float32 and lowres.is_contiguous()
+    B, M, low, _ = lowres.shape
+    H, W = original_size
+    if return_mask and mask is None:
+        mask = torch.empty((B, M, H, W), dtype=torch.bool, device=lowres.device)
+    if return_logits and logits is None:
+        logits = torch.empty((B, M, H, W), dtype=torch.float32, device=lowres.device)
+    L.check(L.load().omg_sam_postprocess(lowres.data_ptr(), B * M, low, mid, int(input_size[0]), int(input_size[1]), H, W,
+                                         float(threshold), _ptr(mask), _ptr(logits), _stream()), "omg_sam_postprocess")
+    return mask, logits
+
+
 def groupnorm(x1, gamma, beta, eps, silu, x2=None, out=None, stats_ws=None):
     """GroupNorm(32)(cat([x1, x2], channel)) [+ SiLU]; x: (B, H, W, C) or (B, HW, C)."""
     _chk16(x1)

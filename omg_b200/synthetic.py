@@ -101,3 +101,38 @@ def make_vae_state_dict(cfg=None, seed: int = 0, device="cpu", dtype=torch.float
             t = torch.randn(shape, generator=g, device=device) * fan_in ** -0.5
         sd[name] = t.to(dtype)
     return sd
+
+
+def make_sam_state_dict(seed: int = 0, device="cpu", dtype=torch.float32) -> Dict[str, torch.Tensor]:
+    """A full EfficientViT-SAM xl1 state dict with random weights: the image encoder's keys and shapes are those of the
+    reference module (tests/golden/sam_xl1_shapes.json, prefixed `image_encoder.`), the prompt encoder's and mask
+    decoder's are segment_anything's [3P] in the configuration of sam.py:520-544 (oracle.sam_decoder.decoder_shapes).
+    Linear / conv weights ~ N(0, 1/fan_in); BatchNorm statistics and norm affines jittered; biases and the learned
+    embeddings small (biases) or unit (token / point embeddings, the Fourier matrix) normal."""
+    import json
+    import os
+    from oracle.sam_decoder import decoder_shapes
+    here = os.path.dirname(os.path.abspath(__file__))
+    with open(os.path.join(here, "..", "tests", "golden", "sam_xl1_shapes.json")) as f:
+        enc = json.load(f)
+    shapes = {"image_encoder." + k: tuple(v) for k, v in enc.items()}
+    shapes.update(decoder_shapes())
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    for k, shp in shapes.items():
+        if k.endswith("running_var"):
+            t = torch.rand(shp, generator=g) + 0.5
+        elif k.endswith("running_mean") or k.endswith(".bias"):
+            t = torch.randn(shp, generator=g) * 0.05
+        elif len(shp) == 1:                                   # norm gamma
+            t = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        elif k.endswith(("embeddings.0.weight", "embeddings.1.weight", "embeddings.2.weight", "embeddings.3.weight",
+                         "_embed.weight", "token.weight", "tokens.weight", "gaussian_matrix")):
+            t = torch.randn(shp, generator=g)
+        else:
+            fan_in = math.prod(shp[1:])
+            if "output_upscaling" in k:                       # ConvTranspose2d weight [in, out, k, k]: fan-in = in
+                fan_in = shp[0]
+            t = torch.randn(shp, generator=g) * fan_in ** -0.5
+        sd[k] = t.to(device, dtype)
+    return sd
