@@ -227,6 +227,10 @@ static int attention_impl(const omg_attn_desc* d, void* stream_) {
     OMG_CHECK(d->q && d->k && d->v && d->out, "omg_attention: null pointer");
     OMG_CHECK(d->out_ld % 8 == 0 && d->out_col0 % 8 == 0 && d->out_bs % 8 == 0,
               "omg_attention: output must be 16 B aligned per row");
+    if (check_head_windows("omg_attention", d->heads, d->head_dim, {d->q_col0, d->k_col0, d->v_col0, d->out_col0},
+                           {d->q_ld, d->k_ld, d->v_ld, d->out_ld}))
+        return 1;
+    OMG_CHECK(!d->causal || (d->n_kv <= 128 && d->n_q <= 128), "omg_attention: causal masking is available for sequences of <= 128 tokens");
     static bool configured = false;
     if (!configured) {
         OMG_CUDA(cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
@@ -265,7 +269,6 @@ static int attention_impl(const omg_attn_desc* d, void* stream_) {
     p.out_weight = d->out_weight;
     p.accumulate = d->accumulate;
     p.causal = d->causal;
-    OMG_CHECK(!d->causal || (d->n_kv <= 128 && d->n_q <= 128), "omg_attention: causal masking is available for sequences of <= 128 tokens");
     dim3 grid((d->n_q + ATT_BQ - 1) / ATT_BQ, d->heads, d->n_items);
     OMG_CUDA(launch_pdl(attn_tc_kernel, grid, dim3(ATT_THREADS), ATT_SMEM, stream, p));
     return check_launch("attn_tc_kernel");

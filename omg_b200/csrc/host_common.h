@@ -27,6 +27,18 @@ inline int fail(const char* fmt, ...) {
         if (!(cond)) return ::omg::fail(__VA_ARGS__); \
     } while (0)
 
+// Attention descriptors (omg_attention, omg_attention_small): the head window [col0, col0 + heads * head_dim) of q, k, v
+// and out must lie inside a row of ld elements, else the kernels read or write the next row, or past the buffer's end.
+inline int check_head_windows(const char* who, int heads, int head_dim, const int (&col0)[4], const int (&ld)[4]) {
+    const char* names[4] = {"q", "k", "v", "out"};
+    const long long width = (long long)heads * head_dim;
+    for (int i = 0; i < 4; ++i)
+        if (col0[i] < 0 || col0[i] + width > ld[i])
+            return fail("%s: %s head window [%d, %lld) does not fit its row of %d elements", who, names[i], col0[i],
+                        col0[i] + width, ld[i]);
+    return 0;
+}
+
 #define OMG_CUDA(expr)                                                                       \
     do {                                                                                     \
         cudaError_t _e = (expr);                                                             \

@@ -300,6 +300,9 @@ static int attention_small_impl(const omg_attn_desc* d, void* ws, void* stream_)
     OMG_CHECK(d->q_ld % 8 == 0 && d->out_ld % 8 == 0 && d->q_col0 % 8 == 0 && d->out_col0 % 8 == 0 && d->q_bs % 8 == 0 &&
                   d->out_bs % 8 == 0 && ((uintptr_t)d->q & 15) == 0 && ((uintptr_t)d->out & 15) == 0,
               "omg_attention_small: q / out rows must be 16 B aligned (ld, col0, batch stride multiples of 8)");
+    if (check_head_windows("omg_attention_small", d->heads, d->head_dim, {d->q_col0, d->k_col0, d->v_col0, d->out_col0},
+                           {d->q_ld, d->k_ld, d->v_ld, d->out_ld}))
+        return 1;
     const omg_attn_desc p = *d;
     const bool d16 = d->head_dim == 16;
     if (d->n_kv <= SA_SHORT) {

@@ -259,6 +259,23 @@ def test_c_abi_rejects_bad_arguments_before_touching_the_gpu():
     assert "head_dim 32 unsupported" in err(lib.omg_attention(C.byref(d), None))
     d.head_dim, d.n_items = 64, 99
     assert "n_items=99 out of range" in err(lib.omg_attention(C.byref(d), None))
+    # head windows (col0 + heads * head_dim) must fit their rows; checked before any CUDA call
+    d.n_items, d.n_q, d.n_kv, d.heads = 1, 16, 16, 2
+    d.q = d.k = d.v = d.out = 0x1000
+    d.q_ld = d.k_ld = d.v_ld = d.out_ld = 128
+    d.q_col0, d.k_col0 = 8, -8
+    assert "q head window [8, 136) does not fit its row of 128" in err(lib.omg_attention(C.byref(d), None))
+    d.q_col0 = 0
+    assert "k head window [-8, 120)" in err(lib.omg_attention(C.byref(d), None))
+    d.k_col0, d.v_ld = 0, 120
+    assert "v head window [0, 128) does not fit its row of 120" in err(lib.omg_attention(C.byref(d), None))
+    d.v_ld, d.out_col0, d.out_ld = 128, 72, 192
+    assert "out head window [72, 200) does not fit its row of 192" in err(lib.omg_attention(C.byref(d), None))
+    d.head_dim, d.heads, d.out_col0, d.out_weight = 32, 4, 0, 1.0
+    d.q_ld = 120
+    assert "omg_attention_small: q head window [0, 128)" in err(lib.omg_attention_small(C.byref(d), None, None))
+    d.q_ld, d.v_col0 = 128, 8
+    assert "v head window [8, 136)" in err(lib.omg_attention_small(C.byref(d), None, None))
     assert "null descriptor" in err(lib.omg_gemm(None, None))
     g = L.GemmDesc()
     g.n_a = 0

@@ -30,7 +30,8 @@ def ops():
                                       (308, 2560, 2048, 0), (4, 1280, 2816, 0), (512, 320, 960, 160),
                                       (512, 320, 960, 64), (2048, 1920, 640, 128), (2048, 1280, 640, 256),
                                       (4096, 1280, 1280, 320), (512, 640, 1024, 320), (300, 320, 640, 320),
-                                      (2176, 960, 192, 320)])
+                                      (2176, 960, 192, 320), (129, 224, 40, 64), (383, 352, 200, 128),
+                                      (127, 224, 1000, 160), (1, 288, 8, 256)])
 def test_linear(ops, M, N, K, bn):
     x, w, b = rnd(M, K, seed=1), rnd(N, K, scale=K ** -0.5, seed=2), rnd(N, seed=3)
     r = rnd(M, N, seed=4)
@@ -155,10 +156,12 @@ def test_self_attention(ops, B, N, heads):
 
 
 @pytest.mark.parametrize("n_q,n_kv,gain", [(256, 200, 1.0), (130, 321, 1.0), (512, 640, 2.5), (128, 129, 2.5),
-                                            (384, 1024, 3.0), (121, 121, 1.0), (200, 57, 1.0), (64, 63, 2.5)])
+                                            (384, 1024, 3.0), (121, 121, 1.0), (200, 57, 1.0), (64, 63, 2.5),
+                                            (1, 1, 1.0), (129, 1, 2.5), (65, 65, 4.0)])
 def test_attention_block_edges(ops, n_q, n_kv, gain):
-    """Self-attention kernel edges: odd block counts, a partial last block, n_q != n_kv, and score ranges large enough
-    that the lazy O rescale fires; with and without `accumulate`."""
+    """attn_tc_kernel edges: odd key-block counts, a partial last block, n_q != n_kv, a single key, and score ranges
+    large enough that the running maximum moves between key blocks (O is rescaled eagerly, at every block); with and
+    without `accumulate`."""
     heads = 3
     Cc = heads * 64
     q = rnd(2, n_q, Cc, seed=11) * gain
@@ -179,8 +182,9 @@ def test_attention_block_edges(ops, n_q, n_kv, gain):
                                               (2, 300, 100, 5), (1, 64, 5, 1), (8, 1024, 77, 20), (2, 256, 57, 3),
                                               (1, 130, 121, 2), (1, 100, 59, 1)])
 def test_cross_attention_head_group_kernel(ops, B, n_q, n_kv, heads):
-    """Cross-attention kernel (one key block, a CTA walks a group of heads): text keys (77), IP tokens (16), padded key
-    counts, ragged query tiles, head counts with a tail group; remapped rows and the accumulate / out_weight term."""
+    """Cross-attention shapes on attn_tc_kernel (the one attention kernel; a CTA per item, head and 128-query tile):
+    text keys (77), IP tokens (16), key counts that leave a partial 64-key block, ragged query tiles, odd head counts;
+    remapped rows and the accumulate / out_weight term."""
     Cc = heads * 64
     q = rnd(B, n_q, Cc, seed=21)
     kv = rnd(B + 1, n_kv, 2 * Cc, seed=22)
@@ -198,9 +202,9 @@ def test_cross_attention_head_group_kernel(ops, B, n_q, n_kv, heads):
 
 @pytest.mark.parametrize("B,N,n_kv,heads", [(4, 1024, 1024, 20), (2, 2048, 320, 8), (3, 640, 200, 5), (1, 4096, 4096, 3)])
 def test_self_attention_persistent_many_tiles(ops, B, N, n_kv, heads):
-    """The persistent self-attention kernel: 2 x #SM CTAs walk several tiles each as one stream of KV blocks (barrier
-    phases run across tile boundaries, Q double-buffered, O handed back through o_free): more tiles than CTAs, odd block
-    counts per tile, a partial last block, remapped batch rows and the accumulate term."""
+    """attn_tc_kernel at many query tiles: more (item, head, 128-query tile) CTAs than fit on the GPU at once, each
+    streaming its key blocks through the 4-stage ring; odd block counts, a partial last block, remapped batch rows and
+    the accumulate term."""
     Cc = heads * 64
     q = rnd(B, N, Cc, seed=41) * 1.5
     kv = rnd(B, n_kv, 2 * Cc, seed=42)
