@@ -8,7 +8,8 @@
  * error string.  Every function returns 0 on success, non-zero on failure (omg_last_error() gives
  * the message); nothing throws across the boundary.  All kernels are launched on the CUstream /
  * cudaStream_t handle passed as `stream` (void*), never synchronise the host, and are CUDA-graph
- * capturable.  fp16 storage, fp32 accumulation.  Activations are channels-last:
+ * capturable.  fp16 storage, fp32 accumulation; omg_gemm (dtype = OMG_DTYPE_BF16), omg_groupnorm_bf16 and
+ * omg_softmax_rows_bf16 also take bf16 storage (the VAE decoder's path).  Activations are channels-last:
  * (B, H, W, C) == (B, H*W tokens, C).
  */
 #ifndef OMG_B200_H
@@ -36,6 +37,9 @@ typedef struct {
     int32_t a_idx, dx, dy, a_c0, k_len, b_k0;
     int32_t b_idx; /* 0: columns of w, 1: columns of w2 (e.g. the LoRA up-projection B, kept un-merged) */
 } omg_seg;
+
+/* Storage type of a descriptor's 16-bit operands (omg_gemm_desc.dtype). */
+enum { OMG_DTYPE_F16 = 0, OMG_DTYPE_BF16 = 1 };
 
 enum { OMG_EPI_NONE = 0, OMG_EPI_GEGLU = 1, OMG_EPI_SILU = 2, OMG_EPI_QUICK_GELU = 3, OMG_EPI_GELU = 4, OMG_EPI_GELU_TANH = 5,
        OMG_EPI_RELU = 6 };
@@ -107,6 +111,11 @@ typedef struct {
     int64_t residual_f32_ld;
     void* out_f32;
     int64_t out_f32_ld;
+    /* Storage type of the A views, w, bias, residual and the output: OMG_DTYPE_F16 (0, so a zeroed descriptor is fp16)
+     * or OMG_DTYPE_BF16.  bf16 covers what the VAE decoder needs - OMG_EPI_NONE with bias and residual, every block_n
+     * and tall tiles - and rejects GEGLU, activation epilogues, rowvec, w2, weight planes, the folded LayerNorm, row and
+     * column statistics and the fp32 twins.  Accumulation is fp32 either way. */
+    int32_t dtype;
 } omg_gemm_desc;
 
 int omg_gemm(const omg_gemm_desc* desc, void* stream);
@@ -158,6 +167,9 @@ int omg_attention(const omg_attn_desc* desc, void* stream);
 #define OMG_GN_WS_FLOATS(B) ((B) * (2 * 2 * 2560 + 64 * OMG_GN_MAX_SPLITS))
 int omg_groupnorm(const void* x1, int C1, const void* x2, int C2, int B, int HW, const void* gamma, const void* beta,
                   float eps, int silu, void* stats_ws, void* y, void* stream);
+/* omg_groupnorm over bf16 x1 / x2 / gamma / beta / y: same arguments, limits, fp32 statistics and summation order. */
+int omg_groupnorm_bf16(const void* x1, int C1, const void* x2, int C2, int B, int HW, const void* gamma, const void* beta,
+                       float eps, int silu, void* stats_ws, void* y, void* stream);
 
 /* Per-channel (sum, sum of squares) partials of a stored channels-last tensor x [B, HW, C], one float2 per channel per
  * 32-row block: out [B][ceil(HW/32)][C] - the layout omg_gemm's col_stats_out produces (for tensors that were modified
@@ -220,6 +232,8 @@ int omg_axpy(const void* a, const void* b, float alpha, void* y, long long n, vo
  * 512 channels: `Attention(heads=1)` inside diffusers' AutoencoderKL, reached from src/pipelines/lora_pipeline.py:649)
  * materialises its scores with omg_gemm, normalises them here and applies them with a second omg_gemm. */
 int omg_softmax_rows(void* x, long long rows, int cols, long long ld, float scale, void* stream);
+/* omg_softmax_rows over a bf16 matrix: same arguments and limits, fp32 arithmetic. */
+int omg_softmax_rows_bf16(void* x, long long rows, int cols, long long ld, float scale, void* stream);
 
 /*
  * EfficientViT-SAM image encoder (the segmentation model between the two stages; SURVEY 8f-4), the ops that are not

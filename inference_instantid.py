@@ -2,15 +2,19 @@
 """OMG + InstantID multi-identity generation on the H100 path.  The reference CLI's flags (names, defaults, types:
 inference_instantid.py:259-286, pinned by tests/golden/cli_flags.json), prompt mini-DSL, two-stage flow and output
 files; additions (non-breaking): --synthetic, --tiny, --num_inference_steps, --image_size, --dedup, --mask_boxes,
---face_embeds, --face_kps, --sam_boxes.
+--face_embeds, --face_kps, --sam_boxes, --decode.
 
-Face analysis (insightface antelopev2), segmentation and the VAE sit outside the accelerated hot path (SURVEY section
-8): when `insightface` is not importable the identities come from --face_embeds (one 512-d .pt / .npy per region) and
-the stage-2 key-points from --face_kps; regions come from --mask_boxes.  In --synthetic mode identities are unit-norm
-random 512-d embeddings (seeds 1, 2), the IdentityNet condition is the reference's `draw_kps_multi` rendering of fixed
-key-points and the masks are the config rectangles.  --sam_boxes (EfficientViT-SAM masks from box prompts, see
-inference_lora.py) needs a decoded stage-1 image; this CLI keeps its stage-1 output as latents, so the flag is checked
-against --mask_boxes and then refused with that reason.
+Face analysis (insightface antelopev2) and detection sit outside the accelerated hot path (SURVEY section 8): when
+`insightface` is not importable the identities come from --face_embeds (one 512-d .pt / .npy per region) and the
+stage-2 key-points from --face_kps; regions come from --mask_boxes or --sam_boxes.  In --synthetic mode identities are
+unit-norm random 512-d embeddings (seeds 1, 2), the IdentityNet condition is the reference's `draw_kps_multi` rendering
+of fixed key-points and the masks are the config rectangles.
+
+Output: with --decode the VAE decodes both stages to stage-1.png / stage-2.png as the reference writes them - the
+checkpoint's own VAE (<pretrained_model>/vae) in bf16, whose exponent range holds activations that overflow fp16 with
+SDXL's VAE weights, or a random-init VAE with --synthetic.  Then --sam_boxes (EfficientViT-SAM masks from box prompts on
+the decoded stage-1 image, see inference_lora.py) replaces the stage-2 region masks.  Without --decode the latents are
+saved (stage-{1,2}.pt) and --sam_boxes is refused.
 """
 import argparse
 import math
@@ -98,6 +102,8 @@ def parse_args():
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
     p.add_argument("--sam_boxes", default="", type=str, help="x0,y0,x1,y1|... box prompts for EfficientViT-SAM on the "
                    "decoded stage-1 image (needs a decoded image; excludes --mask_boxes)")
+    p.add_argument("--decode", action="store_true", help="decode to PNG: <pretrained_model>/vae in bf16 (with "
+                   "--synthetic: a random-init VAE decoder)")
     p.add_argument("--face_embeds", default="", type=str, help="a.pt|b.pt: 512-d identity embeddings, one per region "
                    "(replaces insightface on the reference images)")
     p.add_argument("--face_kps", default="", type=str, help="JSON file: list of five (x, y) key-points per face for "
@@ -247,14 +253,41 @@ if __name__ == "__main__":
             masks.append(m)
         masks = masks or [None] * len(regions)
     pipe.dedup = args.dedup
-    from omg_b200.sam import check_sam_flags
-    check_sam_flags(args.sam_boxes, args.mask_boxes, decoded=getattr(pipe, "vae_decoder", None) is not None)
+    if args.decode:
+        from omg_b200.vae import PackedVaeDecoder, VaeConfig
+        if args.synthetic:
+            vcfg = VaeConfig.tiny() if args.tiny else VaeConfig.sdxl()
+            pipe.vae_decoder = PackedVaeDecoder(synthetic.make_vae_state_dict(vcfg, 0), vcfg, device=device)
+        else:  # the checkpoint's own VAE in bf16, where the reference up-casts to fp32
+            pipe.vae_decoder = PackedVaeDecoder.from_pretrained(args.pretrained_model, "vae", dtype=torch.bfloat16,
+                                                                device=device)
+        kwargs["output_type"] = "pil"  # instantid_pipeline.py: VAE decode + postprocess
+    decoded = pipe.vae_decoder is not None
+    from omg_b200 import sam as sam_lib
+    sam_lib.check_sam_flags(args.sam_boxes, args.mask_boxes, decoded=decoded)
+    sam_boxes = None
+    if args.sam_boxes:
+        try:
+            sam_boxes = sam_lib.parse_sam_boxes(args.sam_boxes)
+        except ValueError as e:
+            raise SystemExit(str(e))
+        if len(sam_boxes) != len(regions):
+            raise SystemExit(f"--sam_boxes has {len(sam_boxes)} entries for {len(regions)} regions")
     input_prompt = [prompts, regions]
     common = dict(input_prompt=input_prompt, concept_models=cm, input_neg_prompt=[args.negative_prompt] * len(input_prompt),
                   controller=controller, face_app=face_app, controlnet_conditioning_scale=args.IdentityNet_rate,
                   guidance_scale=args.cfg_scale, face_embeds=faces, **kwargs)
     image = sample_image(pipe, generator=torch.Generator(device).manual_seed(args.seed), stage=1, **common)
     controller.reset()
+    if sam_boxes is not None:
+        # EfficientViT-SAM on the decoded stage-1 image, one box per region (as inference_lora.py does)
+        if args.synthetic:
+            sam_model = sam_lib.create_sam_model("xl1", state_dict=synthetic.make_sam_state_dict(0))
+        else:
+            sam_model = sam_lib.create_sam_model("xl1", weight_url=args.efficientViT_checkpoint)
+        masks = sam_lib.sam_region_masks(sam_lib.EfficientViTSamPredictor(sam_model), image[0], sam_boxes)
+        for k, m in enumerate(masks):
+            print(f"SAM mask {k}: " + ("no box, region skipped" if m is None else f"{int(m.sum())} pixels"))
     if any(m is not None for m in masks):
         if kps is None:
             raise SystemExit("stage 2 needs the faces' key-points: --face_kps (insightface on the decoded stage-1 image "
@@ -270,6 +303,9 @@ if __name__ == "__main__":
     os.makedirs(save_dir, exist_ok=True)
     print(f"save to: {save_dir}")
     for idx, name in ((0, "stage-1"), (1, "stage-2")):
-        torch.save(image[idx].cpu(), os.path.join(save_dir, name + ".pt"))
+        if decoded:
+            image[idx].save(os.path.join(save_dir, name + ".png"))
+        else:
+            torch.save(image[idx].cpu(), os.path.join(save_dir, name + ".pt"))
     with open(os.path.join(save_dir, f"**---{args.suffix}---{hash_code}.txt"), "w") as fw:
         fw.writelines(configs)

@@ -6,10 +6,15 @@ files as the reference CLI (inference_lora.py:201-323); additions (non-breaking)
 Masks between the stages: with --sam_boxes (x0,y0,x1,y1 per concept, '|' separated, stage-1 pixels) the boxes prompt
 EfficientViT-SAM xl1 on the decoded stage-1 image, as the reference's predict_mask does with a detector's box
 (inference_lora.py:91-126), and the device masks go straight into stage 2 (weights from --efficientViT_checkpoint, or
-random with --synthetic; needs a decoded image: --vae_fp16_safe or --synthetic --decode).  The detectors (YOLO-World /
+random with --synthetic; needs a decoded image: --decode or --vae_fp16_safe).  The detectors (YOLO-World /
 GroundingDINO) stay outside: boxes are an input.  --mask_boxes instead fills the boxes as rectangles; in --synthetic mode
-without either flag the masks are the fixed config-2 rectangles.  Without a VAE the latents are saved (stage-{1,2}.pt)
-next to a PNG visualisation of their first three channels.
+without either flag the masks are the fixed config-2 rectangles.
+
+Output: with --decode the checkpoint's own VAE (<pretrained_sdxl_model>/vae, the original SDXL weights) decodes in bf16,
+whose exponent range holds the activations that overflow fp16, and stage-1.png / stage-2.png are written as the
+reference writes them; --vae_fp16_safe DIR instead decodes the fp16-safe re-export of the VAE in fp16; --synthetic
+--decode uses a random-init VAE.  Without a VAE the latents are saved (stage-{1,2}.pt) next to a PNG visualisation of
+their first three channels.
 """
 import argparse
 import hashlib
@@ -73,7 +78,8 @@ def parse_args():
     p.add_argument("--num_inference_steps", default=50, type=int)
     p.add_argument("--image_size", default=1024, type=int)
     p.add_argument("--tiny", action="store_true", help="with --synthetic: toy widths (plumbing check)")
-    p.add_argument("--decode", action="store_true", help="with --synthetic: decode with a random-init VAE decoder")
+    p.add_argument("--decode", action="store_true", help="decode to PNG: <pretrained_sdxl_model>/vae in bf16 (with "
+                   "--synthetic: a random-init VAE decoder)")
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
     p.add_argument("--vae_fp16_safe", default="", type=str, help="directory of fp16-safe SDXL VAE weights: decode to "
                    "PNG on the GPU (without it the latents are saved)")
@@ -81,6 +87,13 @@ def parse_args():
                    "empty = skip the concept): box prompts for EfficientViT-SAM on the decoded stage-1 image, whose masks "
                    "drive stage 2; needs a decoded image, excludes --mask_boxes")
     return p.parse_args()
+
+
+def check_decode_flags(args):
+    """--decode (the checkpoint's VAE in bf16) and --vae_fp16_safe (another VAE in fp16) name two different decoders."""
+    if args.decode and args.vae_fp16_safe:
+        raise SystemExit("--decode and --vae_fp16_safe are exclusive: --decode decodes <pretrained_sdxl_model>/vae in "
+                         "bf16, --vae_fp16_safe DIR decodes the fp16-safe VAE in DIR in fp16")
 
 
 def _latents_png(lat, path):
@@ -102,8 +115,9 @@ def build_model_synthetic(args, prompts, device):
 def build_model_sd(args, prompts, device):
     """Real checkpoints, mirroring the reference's build_model_sd (inference_lora.py:150-171): the diffusers-layout
     UNet / ControlNet safetensors load straight into PackedUNet, the LoRA files (kohya / SGM / diffusers layouts) through
-    omg_b200.checkpoints, the prompts through the two CLIP towers (omg_b200.text).  Segmentation and the VAE are
-    outside the path: regions come from --mask_boxes and the outputs are latents."""
+    omg_b200.checkpoints, the prompts through the two CLIP towers (omg_b200.text).  Detection is outside the path:
+    regions come from --mask_boxes or --sam_boxes.  The VAE decodes with --decode or --vae_fp16_safe, else the outputs
+    are latents."""
     from omg_b200 import checkpoints as ck
     from omg_b200.config import UNetConfig
     from omg_b200.pipelines import ConceptModels, LoraMultiConceptPipeline, revise_regionally_controlnet_forward
@@ -126,6 +140,10 @@ def build_model_sd(args, prompts, device):
         vae_dir = args.vae_fp16_safe
         sub = "vae" if os.path.isdir(os.path.join(vae_dir, "vae")) else ""
         vae = PackedVaeDecoder(ck.load_unet_weights(vae_dir, sub, None), device=device)
+    elif args.decode:
+        # the checkpoint's own VAE (the original SDXL weights) in bf16, where the reference up-casts to fp32
+        from omg_b200.vae import PackedVaeDecoder
+        vae = PackedVaeDecoder.from_pretrained(args.pretrained_sdxl_model, "vae", dtype=torch.bfloat16, device=device)
     pipe = LoraMultiConceptPipeline(unet, controlnet=controlnet, prompt_encoder=enc, vae_decoder=vae)
     controller = AttentionReplace(prompts, 50, cross_replace_steps={"default_": 1.}, self_replace_steps=0.4,
                                   tokenizer=enc.tokenizer, width=args.image_size // 32, height=args.image_size // 32)
@@ -146,6 +164,7 @@ def build_model_sd(args, prompts, device):
 
 if __name__ == "__main__":
     args = parse_args()
+    check_decode_flags(args)
     if not torch.cuda.is_available():
         raise SystemExit("the H100 path needs a CUDA device (there is no CPU fallback)")
     device = torch.device("cuda")

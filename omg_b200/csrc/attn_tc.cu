@@ -210,7 +210,7 @@ static int make_attn_map(CUtensorMap* m, const void* ptr, int cols, int ld, int 
     const uint64_t dims[3] = {(uint64_t)cols, (uint64_t)tokens, (uint64_t)nb};
     const uint64_t strides[3] = {1, (uint64_t)ld, (uint64_t)bs};
     const uint32_t box[3] = {64, box_rows, 1};
-    return make_tmap_f16(m, ptr, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace omg

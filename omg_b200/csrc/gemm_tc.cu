@@ -20,8 +20,10 @@
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/omg_b200.h"
+#include "elem.cuh"
 #include "host_common.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
@@ -45,12 +47,13 @@ struct alignas(64) GemmParams {
     int tw, th, tiles_w, tiles_h;
     int img_w, img_h, img_b;
     int N, N_out;
-    __half* out;               // output view (channels-last, element strides)
+    // 16-bit operands in the kernel's storage type (fp16 | bf16, omg_gemm_desc.dtype)
+    void* out;                 // output view (channels-last, element strides)
     long long out_sw, out_sh, out_sb;
-    const __half* bias;
-    const __half* rowvec;
+    const void* bias;
+    const void* rowvec;
     int rowvec_ld;
-    const __half* residual;
+    const void* residual;
     int residual_ld;
     int act_silu;
     // LayerNorm folded into the GEMM pair (see omg_gemm_desc): statistics written by the producer's epilogue ...
@@ -100,12 +103,19 @@ struct GemmCfg {
 // GEGLU / erf-GELU use libdevice's erff.
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
-template <int WN>
+template <typename T, int WN>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db) {
-    if constexpr (WN == 64) wgmma_ss_n64(*reinterpret_cast<float(*)[32]>(d), da, db, 1u);
-    else if constexpr (WN == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(d), da, db, 1u);
-    else if constexpr (WN == 160) wgmma_ss_n160(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
-    else wgmma_ss_n256(*reinterpret_cast<float(*)[128]>(d), da, db, 1u);
+    if constexpr (std::is_same_v<T, __nv_bfloat16>) {
+        if constexpr (WN == 64) wgmma_ss_n64_bf16(*reinterpret_cast<float(*)[32]>(d), da, db, 1u);
+        else if constexpr (WN == 128) wgmma_ss_n128_bf16(*reinterpret_cast<float(*)[64]>(d), da, db, 1u);
+        else if constexpr (WN == 160) wgmma_ss_n160_bf16(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
+        else wgmma_ss_n256_bf16(*reinterpret_cast<float(*)[128]>(d), da, db, 1u);
+    } else {
+        if constexpr (WN == 64) wgmma_ss_n64(*reinterpret_cast<float(*)[32]>(d), da, db, 1u);
+        else if constexpr (WN == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(d), da, db, 1u);
+        else if constexpr (WN == 160) wgmma_ss_n160(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
+        else wgmma_ss_n256(*reinterpret_cast<float(*)[128]>(d), da, db, 1u);
+    }
 }
 
 // FEAT selects what the epilogue carries besides bias / time-embedding vector / residual / LayerNorm fold / row statistics:
@@ -113,8 +123,11 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db) {
 //   1  + GroupNorm column statistics (convs, proj_out)
 //   2  + activations (SiLU, quick-GELU, erf / tanh GELU) and the fp32 residual-trunk twins (once-per-call MLPs, CLIP / SAM
 //      towers, OMG_TRUNK_F32)
-template <int BN, int EPI, int MT, int FEAT>
+// T is the storage type of A, W, bias, rowvec, residual and the output (__half, or __nv_bfloat16 for the lean
+// OMG_EPI_NONE instantiations the VAE decoder uses).
+template <typename T, int BN, int EPI, int MT, int FEAT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+    using T2 = pair_t<T>;
     constexpr bool kStats = FEAT >= 1, kExtra = FEAT >= 2;
     static_assert(EPI != OMG_EPI_GEGLU || (BN <= 256 && MT == 1), "GEGLU runs on single 128-row tiles");
     using Cfg = GemmCfg<BN, MT, kStats>;
@@ -230,8 +243,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                         v = p.col_c2[cg + n];
                         c1 = p.col_c1[cg + n];
                     } else {
-                        if (p.bias) v += __half2float(p.bias[n]);
-                        if (p.rowvec && b < p.img_b) v += __half2float(p.rowvec[(size_t)b * p.rowvec_ld + n]);
+                        if (p.bias) v += to_f32(static_cast<const T*>(p.bias)[n]);
+                        if (p.rowvec && b < p.img_b) v += to_f32(static_cast<const T*>(p.rowvec)[(size_t)b * p.rowvec_ld + n]);
                     }
                 }
                 s_bias[sub * BN + j] = v;
@@ -259,7 +272,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
                         for (int nw = 0; nw < Cfg::NW; ++nw) {
                             const uint64_t b_desc = gmma_desc_sw128(b_addr + nw * (Cfg::WN * BK * 2) + k * 32, 1024, 16);
-                            wgmma_ss<Cfg::WN>(acc + i * (BN / 2) + nw * (Cfg::WN / 2), a_desc, b_desc);
+                            wgmma_ss<T, Cfg::WN>(acc + i * (BN / 2) + nw * (Cfg::WN / 2), a_desc, b_desc);
                         }
                     }
                 }
@@ -292,7 +305,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
             float row_sum[2] = {0.f, 0.f}, row_sq[2] = {0.f, 0.f};
             bool valid[2];
             size_t pix[2];
-            __half* orow[2];
+            T* orow[2];
             float ln_a[2] = {1.f, 1.f}, ln_k[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -300,7 +313,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 const int ph = h0 + et / p.tw, pw = w0 + et % p.tw;
                 valid[h] = (ph < p.img_h) && (pw < p.img_w) && (b < p.img_b);
                 pix[h] = ((size_t)b * p.img_h + ph) * p.img_w + pw;
-                orow[h] = p.out + (long long)b * p.out_sb + (long long)ph * p.out_sh + (long long)pw * p.out_sw;
+                orow[h] = static_cast<T*>(p.out) + (long long)b * p.out_sb + (long long)ph * p.out_sh + (long long)pw * p.out_sw;
                 // folded LayerNorm: this row's mean / rstd from the producer's partial sums;
                 // out = ln_a * acc + (ln_k * c1 + c2), ln_k = -rstd * mean
                 if (ln && valid[h]) {
@@ -336,7 +349,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                         const float o = x[h][0] * gelu_exact(x[h][1]);
                         const float o_nb = __shfl_down_sync(0xffffffffu, o, 1);
                         if ((c & 1) == 0 && valid[h] && n < p.N)
-                            *reinterpret_cast<__half2*>(orow[h] + (n >> 1)) = __floats2half2_rn(o, o_nb);
+                            *reinterpret_cast<T2*>(orow[h] + (n >> 1)) = from_f32x2<T>(o, o_nb);
                     }
                 } else {
                     if constexpr (kExtra) {
@@ -365,7 +378,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                     for (int h = 0; h < 2; ++h) {
                         const bool ok = valid[h] && n < p.N;
                         if (ok && p.residual != nullptr) {
-                            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix[h] * (size_t)p.residual_ld + n));
+                            const float2 r = to_f32x2(*reinterpret_cast<const T2*>(static_cast<const T*>(p.residual) + pix[h] * (size_t)p.residual_ld + n));
                             x[h][0] += r.x;
                             x[h][1] += r.y;
                         }
@@ -382,10 +395,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                             row_sum[h] += x[h][0] + x[h][1];
                             row_sq[h] = fmaf(x[h][0], x[h][0], fmaf(x[h][1], x[h][1], row_sq[h]));
                         }
-                        const __half2 o = __floats2half2_rn(x[h][0], x[h][1]);
-                        if (ok) *reinterpret_cast<__half2*>(orow[h] + n) = o;
+                        const T2 o = from_f32x2<T>(x[h][0], x[h][1]);
+                        if (ok) *reinterpret_cast<T2*>(orow[h] + n) = o;
                         if constexpr (kStats) {  // of the fp16-rounded values the consumer GroupNorm will see; rows outside the image count as zeros
-                            const float2 f = valid[h] ? __half22float2(o) : make_float2(0.f, 0.f);
+                            const float2 f = valid[h] ? to_f32x2(o) : make_float2(0.f, 0.f);
                             cs.x += f.x;
                             cs.y = fmaf(f.x, f.x, cs.y);
                             cs.z += f.y;
@@ -447,21 +460,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 }
 
 // ------------------------------------------------------------------------------------------------ host
-static int view_to_tmap(CUtensorMap* m, const omg_view4& v, uint32_t box_c, uint32_t box_w, uint32_t box_h,
-                        CUtensorMapSwizzle sw) {
+static int view_to_tmap(CUtensorMap* m, const omg_view4& v, CUtensorMapDataType dt, uint32_t box_c, uint32_t box_w,
+                        uint32_t box_h, CUtensorMapSwizzle sw) {
     const uint64_t dims[4] = {(uint64_t)v.C, (uint64_t)v.W, (uint64_t)v.H, (uint64_t)v.B};
     const uint64_t strides[4] = {1, (uint64_t)v.sw, (uint64_t)v.sh, (uint64_t)v.sb};
     const uint32_t box[4] = {box_c, box_w, box_h, 1};
-    return make_tmap_f16(m, v.ptr, 4, dims, strides, box, sw);
+    return make_tmap(m, dt, v.ptr, 4, dims, strides, box, sw);
 }
 
-template <int BN, int EPI, int MT, int FEAT>
+template <typename T, int BN, int EPI, int MT, int FEAT>
 static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
     using Cfg = GemmCfg<BN, MT, (FEAT >= 1)>;
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
-        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, MT, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, BN, EPI, MT, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       Cfg::SMEM_BYTES));
         int dev = 0;
         OMG_CUDA(cudaGetDevice(&dev));
@@ -470,7 +483,7 @@ static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
     }
     const int units = ((p.m_tiles + MT - 1) / MT) * p.n_tiles;
     const int grid = std::min(units, num_sms);
-    OMG_CUDA(launch_pdl(gemm_tc_kernel<BN, EPI, MT, FEAT>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
+    OMG_CUDA(launch_pdl(gemm_tc_kernel<T, BN, EPI, MT, FEAT>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
     return check_launch("gemm_tc_kernel");
 }
 
@@ -478,11 +491,11 @@ static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
 template <int BN, int EPI, int MT = 1>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     if constexpr (EPI == OMG_EPI_GEGLU) {
-        return launch_gemm_f<BN, EPI, MT, 0>(p, stream);
+        return launch_gemm_f<__half, BN, EPI, MT, 0>(p, stream);
     } else {
-        if (p.act_silu != 0 || p.residual_f32 != nullptr || p.out_f32 != nullptr) return launch_gemm_f<BN, EPI, MT, 2>(p, stream);
-        if (p.col_stats != nullptr) return launch_gemm_f<BN, EPI, MT, 1>(p, stream);
-        return launch_gemm_f<BN, EPI, MT, 0>(p, stream);
+        if (p.act_silu != 0 || p.residual_f32 != nullptr || p.out_f32 != nullptr) return launch_gemm_f<__half, BN, EPI, MT, 2>(p, stream);
+        if (p.col_stats != nullptr) return launch_gemm_f<__half, BN, EPI, MT, 1>(p, stream);
+        return launch_gemm_f<__half, BN, EPI, MT, 0>(p, stream);
     }
 }
 
@@ -558,6 +571,20 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     OMG_CHECK(d->w && d->d.ptr, "omg_gemm: null weight/output pointer");
     OMG_CHECK(d->N >= 8 && d->N % 8 == 0, "omg_gemm: N=%d must be a positive multiple of 8", d->N);
     OMG_CHECK(d->Ktot % 8 == 0, "omg_gemm: Ktot=%d must be a multiple of 8", d->Ktot);
+    OMG_CHECK(d->dtype == OMG_DTYPE_F16 || d->dtype == OMG_DTYPE_BF16, "omg_gemm: dtype=%d unsupported (0 fp16, 1 bf16)",
+              d->dtype);
+    const bool bf16 = d->dtype == OMG_DTYPE_BF16;
+    if (bf16) {  // the bf16 instantiations are the lean ones: bias and residual, no other epilogue feature
+        OMG_CHECK(d->epilogue == OMG_EPI_NONE, "omg_gemm: bf16 supports only OMG_EPI_NONE (epilogue %d)", d->epilogue);
+        OMG_CHECK(!d->rowvec, "omg_gemm: bf16 does not support rowvec");
+        OMG_CHECK(!d->w2, "omg_gemm: bf16 does not support a second weight matrix (w2)");
+        OMG_CHECK(d->w_group_planes == 0, "omg_gemm: bf16 does not support weight planes");
+        OMG_CHECK(!d->row_stats_in, "omg_gemm: bf16 does not support the folded LayerNorm");
+        OMG_CHECK(!d->row_stats_out, "omg_gemm: bf16 does not support row statistics");
+        OMG_CHECK(!d->col_stats_out, "omg_gemm: bf16 does not support column statistics");
+        OMG_CHECK(!d->residual_f32 && !d->out_f32, "omg_gemm: bf16 does not support fp32 twins");
+    }
+    const CUtensorMapDataType tdt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     const bool geglu = d->epilogue == OMG_EPI_GEGLU;
     const bool silu = d->epilogue == OMG_EPI_SILU;
     const int act = silu ? 1 : (d->epilogue == OMG_EPI_QUICK_GELU ? 2 : (d->epilogue == OMG_EPI_GELU ? 3 : (d->epilogue == OMG_EPI_GELU_TANH ? 4 :
@@ -599,10 +626,10 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
               d->cta_pair);
     if (geglu) bn = 256;
     p.n_tiles = (d->N + bn - 1) / bn;
-    p.bias = static_cast<const __half*>(d->bias);
-    p.rowvec = static_cast<const __half*>(d->rowvec);
+    p.bias = d->bias;
+    p.rowvec = d->rowvec;
     p.rowvec_ld = d->rowvec_ld;
-    p.residual = static_cast<const __half*>(d->residual);
+    p.residual = d->residual;
     p.residual_ld = d->residual_ld;
     p.act_silu = act;  // 0 none, 1 SiLU, 2 quick_gelu, 3 erf-gelu, 4 tanh-gelu, 5 ReLU
     p.stats_out = static_cast<float*>(d->row_stats_out);
@@ -646,7 +673,7 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
 
     for (int i = 0; i < d->n_a; ++i) {
         OMG_CHECK(d->a[i].ptr != nullptr, "omg_gemm: A view %d is null", i);
-        if (view_to_tmap(&p.a_maps[i], d->a[i], BK, tw, th, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+        if (view_to_tmap(&p.a_maps[i], d->a[i], tdt, BK, tw, th, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
     }
     for (int i = d->n_a; i < OMG_MAX_A; ++i) p.a_maps[i] = p.a_maps[0];
     {
@@ -654,7 +681,7 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
         const uint64_t dims[2] = {(uint64_t)d->Ktot, (uint64_t)d->N * planes};
         const uint64_t strides[2] = {1, (uint64_t)d->Ktot};
         const uint32_t box[2] = {BK, (uint32_t)(bn > 256 ? bn / 2 : bn)};
-        if (make_tmap_f16(&p.b_maps[0], d->w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+        if (make_tmap(&p.b_maps[0], tdt, d->w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
         p.b_maps[1] = p.b_maps[0];
     }
     if (d->w2 != nullptr) {
@@ -662,11 +689,11 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
         const uint64_t dims[2] = {(uint64_t)d->K2tot, (uint64_t)d->N};
         const uint64_t strides[2] = {1, (uint64_t)d->K2tot};
         const uint32_t box[2] = {BK, (uint32_t)(bn > 256 ? bn / 2 : bn)};
-        if (make_tmap_f16(&p.b_maps[1], d->w2, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+        if (make_tmap(&p.b_maps[1], tdt, d->w2, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
     }
     OMG_CHECK(d->d.sw % 2 == 0 && d->d.sh % 2 == 0 && d->d.sb % 2 == 0 && (reinterpret_cast<uintptr_t>(d->d.ptr) & 3) == 0,
               "omg_gemm: output view must be 4 B aligned per pixel");
-    p.out = static_cast<__half*>(const_cast<void*>(d->d.ptr));
+    p.out = const_cast<void*>(d->d.ptr);
     p.out_sw = d->d.sw;
     p.out_sh = d->d.sh;
     p.out_sb = d->d.sb;
@@ -692,11 +719,21 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     for (int i = 0; i < p.n_segs; ++i) k_blocks += p.segs[i].k_blocks;
     bool pair_ok = true;  // both m-tiles of a tall tile must belong to the same stream
     for (int i = 0; i + 1 < p.n_col_groups; ++i) pair_ok = pair_ok && (p.col_group_end[i] % 256 == 0);
-    if (bn == 320) return launch_gemm<320, OMG_EPI_NONE>(p, stream);
     // tall tiles (256 x 160 per CTA): the narrow-N, long-enough-K GEMMs
     const bool tall = bn == 160 && !geglu && pair_ok &&
                       (d->cta_pair == 3 ||
                        (d->cta_pair == 0 && (prefer_tall || use_tall_tiles(p.m_tiles, p.n_tiles, k_blocks))));
+    if (bf16) {  // lean (FEAT 0) OMG_EPI_NONE tiles only: every other feature was rejected above
+        if (tall) return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 2, 0>(p, stream);
+        switch (bn) {
+            case 64: return launch_gemm_f<__nv_bfloat16, 64, OMG_EPI_NONE, 1, 0>(p, stream);
+            case 128: return launch_gemm_f<__nv_bfloat16, 128, OMG_EPI_NONE, 1, 0>(p, stream);
+            case 160: return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 1, 0>(p, stream);
+            case 320: return launch_gemm_f<__nv_bfloat16, 320, OMG_EPI_NONE, 1, 0>(p, stream);
+            default: return launch_gemm_f<__nv_bfloat16, 256, OMG_EPI_NONE, 1, 0>(p, stream);
+        }
+    }
+    if (bn == 320) return launch_gemm<320, OMG_EPI_NONE>(p, stream);
     if (tall) return launch_gemm<160, OMG_EPI_NONE, 2>(p, stream);
     if (geglu) return launch_gemm<256, OMG_EPI_GEGLU>(p, stream);
     switch (bn) {

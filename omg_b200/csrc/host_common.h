@@ -103,9 +103,9 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 // libcuda is resolved at run time through the runtime (the build box has no driver library to link against).
 PFN_encodeTiled get_encode_tiled();
 
-// fp16 tensor map of rank `rank` (<=5). dims[0] is the contiguous dimension. strides are in ELEMENTS for
-// dims[1..rank-1].  Out-of-bounds box elements read as zero / are clipped on store.
-int make_tmap_f16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                  const uint32_t* box, CUtensorMapSwizzle swizzle);
+// Tensor map of rank `rank` (<=5) over 2-byte elements of type `dt` (FLOAT16 | BFLOAT16). dims[0] is the contiguous
+// dimension. strides are in ELEMENTS for dims[1..rank-1].  Out-of-bounds box elements read as zero / are clipped on store.
+int make_tmap(CUtensorMap* out, CUtensorMapDataType dt, const void* ptr, int rank, const uint64_t* dims,
+              const uint64_t* strides_elems, const uint32_t* box, CUtensorMapSwizzle swizzle);
 
 }  // namespace omg

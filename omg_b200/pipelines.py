@@ -212,8 +212,9 @@ class _BasePipeline:
                         use_graphs: bool = True, **_):
         """`LoraMultiConceptPipeline.from_pretrained(pretrained_model, controlnet=controlnet, torch_dtype=float16,
         variant="fp16")` (inference_lora.py:154-155, inference_instantid.py:197-198).  controlnet: a PackedUNet, a
-        checkpoint directory, or None.  The VAE is not loaded here: fp16 activations need the fp16-safe VAE weights,
-        so image output is opt-in through `vae_decoder=` (default output is latents)."""
+        checkpoint directory, or None.  The VAE is not loaded here: image output is opt-in through `vae_decoder=`
+        (default output is latents), e.g. `PackedVaeDecoder.from_pretrained(pretrained_model)`, which decodes the
+        checkpoint's own VAE in bf16 (the original SDXL VAE weights overflow fp16 activations)."""
         unet, prompt_encoder = _load_base(pretrained_model, unet, prompt_encoder, torch_dtype, variant, device)
         if isinstance(controlnet, (str, os.PathLike)):
             controlnet = load_controlnet(controlnet, device)

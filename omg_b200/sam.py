@@ -461,8 +461,8 @@ def check_sam_flags(sam_boxes: str, mask_boxes: str, decoded: bool) -> None:
     if mask_boxes:
         raise SystemExit("--sam_boxes and --mask_boxes are exclusive: SAM masks from boxes, or the boxes as rectangles")
     if not decoded:
-        raise SystemExit("--sam_boxes segments the decoded stage-1 image: pass --vae_fp16_safe (real weights) or "
-                         "--synthetic --decode")
+        raise SystemExit("--sam_boxes segments the decoded stage-1 image: pass --decode (with --synthetic: a "
+                         "random-init VAE) or, for the LoRA CLI, --vae_fp16_safe")
 
 
 def sam_region_masks(predictor: "EfficientViTSamPredictor", image, boxes) -> List[Optional[torch.Tensor]]:
