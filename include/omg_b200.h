@@ -286,6 +286,37 @@ int omg_sam_mask_head(const void* up1, const void* ln_w, const void* ln_b, const
 int omg_sam_postprocess(const void* lowres, int BM, int low, int mid, int h_in, int w_in, int H, int W, float threshold,
                         void* mask, void* logits, void* stream);
 
+/*
+ * omg_attention_relpos: segment_anything's ViT image-encoder attention with decomposed relative-position bias
+ * (Attention.forward with use_rel_pos = True, add_decomposed_rel_pos / get_rel_pos [3P]; the original SAM ViT-B/L/H that
+ * the reference's `--segment_type GroundingDINO` branch prompts, inference_lora.py:91-126,191-198), fp32 softmax,
+ * probabilities never materialised:
+ *   S[q, k] = scale q.k + q.Rh[qh - kh + Sh - 1] + q.Rw[qw - kw + Sw - 1]     (the rel-pos terms use the UNSCALED q)
+ *   out = softmax(S) V                                                      per image, head and attention group.
+ * qkv: fp16 [B, H*W, ld] rows in token order (row-major H x W grid) - the qkv Linear's output, head h's q / k / v at
+ * columns q_col0 / k_col0 / v_col0 + head_dim * h.  out: fp16 [B, H*W, out_ld], head h at out_col0 + head_dim * h (what
+ * proj consumes).  head_dim 64 | 80.  rel_pos_h [rel_h_len, head_dim], rel_pos_w [rel_w_len, head_dim] fp16, contiguous.
+ *   window == 0: global attention over the H x W grid (H, W <= 64); rel_h_len = 2H - 1, rel_w_len = 2W - 1.
+ *   window  > 0: window_partition / window_unpartition: the grid is padded at the bottom and right to multiples of the
+ *     window and attention runs inside each window x window group (window <= 64); rel_h_len = rel_w_len = 2 window - 1.
+ *     The reference pads the normalised input before qkv, so a padded key / value is the qkv bias: k_bias / v_bias
+ *     (fp16 [heads * head_dim], head h at head_dim * h) are required when H or W is not a multiple of the window.
+ *     Outputs of padded queries are not written.
+ * No interpolation of the tables (get_rel_pos with unequal sizes) and no batch remapping.
+ */
+typedef struct {
+    const void* qkv; int32_t ld; int64_t bs; int32_t q_col0, k_col0, v_col0;
+    void* out;       int32_t out_ld; int64_t out_bs; int32_t out_col0;
+    int32_t B, H, W, heads, head_dim, window;
+    const void* rel_pos_h; int32_t rel_h_len;
+    const void* rel_pos_w; int32_t rel_w_len;
+    const void* k_bias;
+    const void* v_bias;
+    float scale;      /* head_dim^-0.5 */
+} omg_attn_relpos_desc;
+
+int omg_attention_relpos(const omg_attn_relpos_desc* desc, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Launch plans: a forward as a handle.  The reference drives one UNet forward as a Python call
  * (`self.unet(latent_model_input, t, ...)`, src/pipelines/lora_pipeline.py:558-567, 588-606); a host that is not Python -

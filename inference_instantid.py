@@ -280,12 +280,12 @@ if __name__ == "__main__":
     image = sample_image(pipe, generator=torch.Generator(device).manual_seed(args.seed), stage=1, **common)
     controller.reset()
     if sam_boxes is not None:
-        # EfficientViT-SAM on the decoded stage-1 image, one box per region (as inference_lora.py does)
-        if args.synthetic:
-            sam_model = sam_lib.create_sam_model("xl1", state_dict=synthetic.make_sam_state_dict(0))
-        else:
-            sam_model = sam_lib.create_sam_model("xl1", weight_url=args.efficientViT_checkpoint)
-        masks = sam_lib.sam_region_masks(sam_lib.EfficientViTSamPredictor(sam_model), image[0], sam_boxes)
+        # predict_mask (inference_lora.py:91-126) with the boxes as the detections, on the decoded stage-1 image:
+        # --segment_type GroundingDINO prompts the original SAM (ViT-H, --sam_checkpoint), any other value
+        # EfficientViT-SAM xl1; masks stay on the device
+        predictor = sam_lib.make_segmenter(args.segment_type, args.synthetic, args.tiny, args.efficientViT_checkpoint,
+                                           args.sam_checkpoint)
+        masks = sam_lib.sam_region_masks(predictor, image[0], sam_boxes)
         for k, m in enumerate(masks):
             print(f"SAM mask {k}: " + ("no box, region skipped" if m is None else f"{int(m.sum())} pixels"))
     if any(m is not None for m in masks):

@@ -50,6 +50,16 @@ class AttnDesc(C.Structure):
                 ("scale", C.c_float), ("out_weight", C.c_float), ("accumulate", C.c_int32), ("causal", C.c_int32)]
 
 
+class AttnRelposDesc(C.Structure):
+    _fields_ = [("qkv", C.c_void_p), ("ld", C.c_int32), ("bs", C.c_int64), ("q_col0", C.c_int32), ("k_col0", C.c_int32),
+                ("v_col0", C.c_int32),
+                ("out", C.c_void_p), ("out_ld", C.c_int32), ("out_bs", C.c_int64), ("out_col0", C.c_int32),
+                ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("heads", C.c_int32), ("head_dim", C.c_int32),
+                ("window", C.c_int32),
+                ("rel_pos_h", C.c_void_p), ("rel_h_len", C.c_int32), ("rel_pos_w", C.c_void_p), ("rel_w_len", C.c_int32),
+                ("k_bias", C.c_void_p), ("v_bias", C.c_void_p), ("scale", C.c_float)]
+
+
 class FuseDesc(C.Structure):
     _fields_ = [("noise_main", C.c_void_p), ("noise_concept", C.c_void_p * OMG_MAX_CONCEPTS),
                 ("mask", C.c_void_p * OMG_MAX_CONCEPTS), ("n_concepts", C.c_int32), ("guidance", C.c_float),
@@ -85,6 +95,7 @@ SYMBOLS = {
     "omg_relu_linear_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "omg_resize_bicubic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "omg_attention_small": (C.c_int, [C.POINTER(AttnDesc), C.c_void_p, C.c_void_p]),
+    "omg_attention_relpos": (C.c_int, [C.POINTER(AttnRelposDesc), C.c_void_p]),
     "omg_sam_mask_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
                                     C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "omg_sam_postprocess": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -165,6 +165,16 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
     d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
+// Same descriptor for tiles of [rows][16 fp16] with 32-byte rows written by TMA SWIZZLE_32B (layout 3): one K = 16 slice
+// per row (K-major), or a 16-wide MN extent (MN-major); 8-row groups are 256 B apart (SBO).  Aligned to 256 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw32(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>(256 >> 4) << 16;
+    d |= static_cast<uint64_t>(256 >> 4) << 32;
+    d |= static_cast<uint64_t>(3) << 62;
+    return d;
+}
 // orders this thread's register accesses to accumulators / A fragments before the wgmma that follows
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

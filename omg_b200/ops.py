@@ -310,6 +310,38 @@ def attention_small(q, k, v, out, heads, head_dim, n_q, n_kv, q_col0=0, k_col0=0
     return out
 
 
+def attention_relpos(qkv, H, W, heads, head_dim, rel_pos_h, rel_pos_w, window=0, k_bias=None, v_bias=None, out=None,
+                     q_col0=None, k_col0=None, v_col0=None, out_col0=0, scale=None):
+    """SAM ViT attention with decomposed relative-position bias (omg_attention_relpos).  qkv: fp16 [B, H*W, ld] in token
+    order, q / k / v of head h at columns q_col0 / k_col0 / v_col0 + head_dim * h (default 0, C, 2C: the qkv Linear's
+    output).  rel_pos_h / rel_pos_w: fp16 [2S - 1, head_dim] (S = window, or H / W when window = 0).  k_bias / v_bias:
+    fp16 [C], the qkv bias of k and v - the padded tokens' key and value when H or W is not a multiple of the window.
+    Returns out, fp16 [B, H*W, >= C] (allocated [B, H*W, C] when None)."""
+    Cd = heads * head_dim
+    q_col0 = 0 if q_col0 is None else q_col0
+    k_col0 = Cd if k_col0 is None else k_col0
+    v_col0 = 2 * Cd if v_col0 is None else v_col0
+    for t in (qkv, rel_pos_h, rel_pos_w, k_bias, v_bias, out):
+        if t is not None:
+            _chk16(t)
+    assert qkv.dim() == 3 and qkv.stride(2) == 1 and qkv.shape[1] == H * W
+    for t in (rel_pos_h, rel_pos_w, k_bias, v_bias):
+        assert t is None or t.is_contiguous()
+    if out is None:
+        out = torch.empty(qkv.shape[0], H * W, Cd, dtype=torch.float16, device=qkv.device)
+    assert out.dim() == 3 and out.stride(2) == 1
+    d = L.AttnRelposDesc()
+    d.qkv, d.ld, d.bs, d.q_col0, d.k_col0, d.v_col0 = qkv.data_ptr(), qkv.stride(1), qkv.stride(0), q_col0, k_col0, v_col0
+    d.out, d.out_ld, d.out_bs, d.out_col0 = out.data_ptr(), out.stride(1), out.stride(0), out_col0
+    d.B, d.H, d.W, d.heads, d.head_dim, d.window = qkv.shape[0], H, W, heads, head_dim, window
+    d.rel_pos_h, d.rel_h_len = rel_pos_h.data_ptr(), rel_pos_h.shape[0]
+    d.rel_pos_w, d.rel_w_len = rel_pos_w.data_ptr(), rel_pos_w.shape[0]
+    d.k_bias, d.v_bias = _ptr(k_bias), _ptr(v_bias)
+    d.scale = head_dim ** -0.5 if scale is None else scale
+    L.check(L.load().omg_attention_relpos(C.byref(d), _stream()), "omg_attention_relpos")
+    return out
+
+
 def sam_mask_head(up1, ln_w, ln_b, w2, b2, hyper, M, eps=1e-6, out=None):
     """SAM output_upscaling after ConvTranspose2d #1 + hypernetwork product (omg_sam_mask_head).  up1 fp16
     [B, 64, 64, 2, 2, 64] (or [B*4096, 256]); w2 fp32 [2, 2, 64, 32]; hyper fp16 (B, M, 32) view with unit channel

@@ -437,6 +437,184 @@ class EfficientViTSamPredictor:
         return tuple(t.clone() for t in out)
 
 
+# ------------------------------------------------------------------------------- original SAM (ViT-B / L / H)
+# The segmenter of the reference's `--segment_type GroundingDINO` branch: segment_anything's `sam_model_registry` /
+# `SamPredictor` on `sam_vit_h_4b8939.pth` (inference_lora.py:105,191-198).  The image encoder is omg_b200.sam_vit; the
+# prompt encoder and mask decoder are the same segment_anything modules the EfficientViT-SAM path runs, with the same
+# keys (`prompt_encoder.*`, `mask_decoder.*`).
+class PackedSam(PackedEfficientViTSam):
+    """segment_anything Sam (image encoder ViT, prompt encoder, mask decoder, postprocess) on the kernels.  Its
+    pixel_mean / pixel_std are SAM's (0-255 scale) - the same normalisation as EfficientViT-SAM's ToTensor + Normalize."""
+
+    pixel_mean = (123.675, 116.28, 103.53)
+    pixel_std = (58.395, 57.12, 57.375)
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", use_graph: bool = True):
+        from .sam_vit import PackedSamViTImageEncoder
+        self.device = torch.device(device)
+        self.image_encoder = PackedSamViTImageEncoder(state_dict, device=device, use_graph=use_graph)
+        dec = {k: v.cpu() for k, v in state_dict.items() if k.startswith(("prompt_encoder.", "mask_decoder."))}
+        self.prompt_encoder = PackedSamPromptEncoder(dec, device=device)      # packs from CPU tensors
+        self.mask_decoder = PackedSamMaskDecoder(dec, self.prompt_encoder.dense_pe_cl, device=device)
+        self.image_size = (IMG_SIZE, IMG_SIZE)
+        self.use_graph = use_graph
+        self._no_mask = self.prompt_encoder.no_mask_embed.half().expand(1, IMG_EMB, IMG_EMB, EMBED).contiguous()
+
+
+def _build_sam(kind: str, checkpoint: Optional[str] = None, state_dict: Optional[Dict[str, torch.Tensor]] = None,
+               device="cuda", use_graph: bool = True) -> PackedSam:
+    from .sam_vit import topology_kind
+    if state_dict is None:
+        if checkpoint is None:
+            raise ValueError("the packed model is built from weights: give checkpoint= (or state_dict=)")
+        with open(checkpoint, "rb") as f:
+            state_dict = torch.load(f, map_location="cpu")
+    got = topology_kind(state_dict)
+    if got != kind:
+        raise ValueError(f"checkpoint is a SAM {got} image encoder, not the requested {kind}")
+    return PackedSam(state_dict, device=device, use_graph=use_graph)
+
+
+def build_sam_vit_h(checkpoint=None, **kw) -> PackedSam:
+    return _build_sam("vit_h", checkpoint, **kw)
+
+
+def build_sam_vit_l(checkpoint=None, **kw) -> PackedSam:
+    return _build_sam("vit_l", checkpoint, **kw)
+
+
+def build_sam_vit_b(checkpoint=None, **kw) -> PackedSam:
+    return _build_sam("vit_b", checkpoint, **kw)
+
+
+build_sam = build_sam_vit_h
+sam_model_registry = {"default": build_sam_vit_h, "vit_h": build_sam_vit_h, "vit_l": build_sam_vit_l,
+                      "vit_b": build_sam_vit_b}
+
+
+class ResizeLongestSide:
+    """segment_anything.utils.transforms.ResizeLongestSide [3P]: resize so the long side is target_length (PIL bilinear on
+    uint8 HWC arrays), and map coordinates / boxes from the original frame into that frame."""
+
+    def __init__(self, target_length: int) -> None:
+        self.target_length = target_length
+
+    @staticmethod
+    def get_preprocess_shape(oldh: int, oldw: int, long_side_length: int) -> Tuple[int, int]:
+        return EfficientViTSamPredictor.get_preprocess_shape(oldh, oldw, long_side_length)
+
+    def apply_image(self, image: np.ndarray) -> np.ndarray:
+        from PIL import Image
+        h, w = self.get_preprocess_shape(image.shape[0], image.shape[1], self.target_length)
+        return np.array(Image.fromarray(np.ascontiguousarray(image)).resize((w, h), Image.BILINEAR))
+
+    def apply_coords(self, coords: np.ndarray, original_size) -> np.ndarray:
+        old_h, old_w = original_size
+        new_h, new_w = self.get_preprocess_shape(old_h, old_w, self.target_length)
+        coords = np.array(coords, dtype=float, copy=True)
+        coords[..., 0] = coords[..., 0] * (new_w / old_w)
+        coords[..., 1] = coords[..., 1] * (new_h / old_h)
+        return coords
+
+    def apply_boxes(self, boxes: np.ndarray, original_size) -> np.ndarray:
+        return self.apply_coords(np.asarray(boxes).reshape(-1, 2, 2), original_size).reshape(-1, 4)
+
+    def apply_coords_torch(self, coords: torch.Tensor, original_size) -> torch.Tensor:
+        old_h, old_w = original_size
+        new_h, new_w = self.get_preprocess_shape(old_h, old_w, self.target_length)
+        coords = coords.clone().float()
+        coords[..., 0] = coords[..., 0] * (new_w / old_w)
+        coords[..., 1] = coords[..., 1] * (new_h / old_h)
+        return coords
+
+    def apply_boxes_torch(self, boxes: torch.Tensor, original_size) -> torch.Tensor:
+        return self.apply_coords_torch(boxes.reshape(-1, 2, 2), original_size).reshape(-1, 4)
+
+
+class SamPredictor(EfficientViTSamPredictor):
+    """segment_anything SamPredictor [3P] on the packed model: set_image / set_torch_image / predict / predict_torch /
+    get_image_embedding / reset_image, with `transform` a ResizeLongestSide.  The machinery (prompt graphs,
+    postprocess) is the EfficientViT-SAM predictor's; only segment_anything's surface differs."""
+
+    def __init__(self, sam_model: PackedSam) -> None:
+        super().__init__(sam_model)
+        self._transform = ResizeLongestSide(sam_model.image_size[0])
+
+    @property
+    def transform(self):
+        return self._transform
+
+    def apply_coords(self, coords, im_size=None):
+        return self.transform.apply_coords(coords, self.original_size if im_size is None else im_size)
+
+    def apply_boxes(self, boxes, im_size=None):
+        return self.transform.apply_boxes(boxes, self.original_size if im_size is None else im_size)
+
+    def apply_boxes_torch(self, boxes, im_size=None):
+        return self.transform.apply_boxes_torch(boxes, self.original_size if im_size is None else im_size)
+
+    @torch.inference_mode()
+    def set_image(self, image: np.ndarray, image_format: str = "RGB") -> None:
+        assert image_format in ["RGB", "BGR"], f"image_format must be in ['RGB', 'BGR'], is {image_format}."
+        if image_format != self.model.image_format:
+            image = image[..., ::-1]
+        input_image = self.transform.apply_image(image)
+        x = torch.as_tensor(input_image, device=self.device).permute(2, 0, 1).contiguous()[None, :, :, :]
+        self.set_torch_image(x, image.shape[:2])
+
+    @torch.inference_mode()
+    def set_torch_image(self, transformed_image: torch.Tensor, original_image_size) -> None:
+        """(1, 3, H, W) image already resized so its long side is 1024 (0-255 values) -> normalise, pad, encode."""
+        assert (len(transformed_image.shape) == 4 and transformed_image.shape[1] == 3
+                and max(*transformed_image.shape[2:]) == self.model.image_size[0]), \
+            f"set_torch_image input must be BCHW with long side {self.model.image_size[0]}."
+        self.reset_image()
+        self.original_size = tuple(original_image_size)
+        self.input_size = tuple(transformed_image.shape[-2:])
+        x = transformed_image.to(self.device, torch.float32)
+        mean = torch.tensor(self.model.pixel_mean, device=self.device)[None, :, None, None]
+        std = torch.tensor(self.model.pixel_std, device=self.device)[None, :, None, None]
+        x = (x - mean) / std
+        size = self.model.image_size[0]
+        x = torch.nn.functional.pad(x, (0, size - x.shape[-1], 0, size - x.shape[-2]))
+        self.features = self.model.image_encoder(x)
+        src = self.model.image_src(self.features)
+        if self._src is None:
+            self._src = torch.empty_like(src)
+        self._src.copy_(src)
+        self.is_image_set = True
+
+    def get_image_embedding(self) -> torch.Tensor:
+        if not self.is_image_set:
+            raise RuntimeError("An image must be set with .set_image(...) to generate an embedding.")
+        return self.features
+
+
+def uses_original_sam(segment_type: str) -> bool:
+    """`--segment_type GroundingDINO` prompts the original SAM (ViT-H); any other value keeps EfficientViT-SAM, as the
+    reference's `else` branch does (inference_lora.py:191-198,276-283)."""
+    return segment_type == "GroundingDINO"
+
+
+def make_segmenter(segment_type: str, synthetic: bool, tiny: bool, efficientvit_checkpoint: str, sam_checkpoint: str):
+    """The predictor the CLIs' --sam_boxes prompt: SamPredictor(build_sam(sam_checkpoint)) for GroundingDINO, else
+    EfficientViTSamPredictor(xl1).  --synthetic: random-init weights (ViT-H-shaped, ViT-B-shaped with --tiny)."""
+    from . import synthetic as syn
+    if uses_original_sam(segment_type):
+        if synthetic:
+            kind = "vit_b" if tiny else "vit_h"
+            model = sam_model_registry[kind](state_dict=syn.make_sam_vit_state_dict(kind, 0, device="cuda",
+                                                                                     dtype=torch.float16))
+        else:
+            model = build_sam(checkpoint=sam_checkpoint)
+        return SamPredictor(model)
+    if synthetic:
+        model = create_sam_model("xl1", state_dict=syn.make_sam_state_dict(0))
+    else:
+        model = create_sam_model("xl1", weight_url=efficientvit_checkpoint)
+    return EfficientViTSamPredictor(model)
+
+
 # ------------------------------------------------------------------------------------------------ CLI helpers
 def parse_sam_boxes(spec: str) -> List[Optional[Tuple[float, float, float, float]]]:
     """--sam_boxes "x0,y0,x1,y1|...": one box per concept in stage-1 image pixels; an empty entry is None (that concept
@@ -465,7 +643,7 @@ def check_sam_flags(sam_boxes: str, mask_boxes: str, decoded: bool) -> None:
                          "random-init VAE) or, for the LoRA CLI, --vae_fp16_safe")
 
 
-def sam_region_masks(predictor: "EfficientViTSamPredictor", image, boxes) -> List[Optional[torch.Tensor]]:
+def sam_region_masks(predictor, image, boxes) -> List[Optional[torch.Tensor]]:
     """One device bool mask (H, W) per box (None stays None) of the RGB image (PIL or HWC uint8): set_image once, then
     predict_torch(boxes, multimask_output=False) - the reference's predict_mask (inference_lora.py:91-126) for boxes."""
     predictor.set_image(np.asarray(image), image_format="RGB")
@@ -473,7 +651,8 @@ def sam_region_masks(predictor: "EfficientViTSamPredictor", image, boxes) -> Lis
     out: List[Optional[torch.Tensor]] = [None] * len(boxes)
     if idx:
         bt = torch.tensor([boxes[i] for i in idx], dtype=torch.float32, device=predictor.device)
-        masks, _, _ = predictor.predict_torch(boxes=predictor.apply_boxes_torch(bt), multimask_output=False)
+        masks, _, _ = predictor.predict_torch(boxes=predictor.transform.apply_boxes_torch(bt, predictor.original_size),
+                                              multimask_output=False)
         for j, i in enumerate(idx):
             out[i] = masks[j, 0]
     return out

@@ -118,21 +118,59 @@ def make_sam_state_dict(seed: int = 0, device="cpu", dtype=torch.float32) -> Dic
     shapes = {"image_encoder." + k: tuple(v) for k, v in enc.items()}
     shapes.update(decoder_shapes())
     g = torch.Generator().manual_seed(seed)
-    sd = {}
-    for k, shp in shapes.items():
-        if k.endswith("running_var"):
-            t = torch.rand(shp, generator=g) + 0.5
-        elif k.endswith("running_mean") or k.endswith(".bias"):
-            t = torch.randn(shp, generator=g) * 0.05
-        elif len(shp) == 1:                                   # norm gamma
-            t = 1.0 + 0.1 * torch.randn(shp, generator=g)
-        elif k.endswith(("embeddings.0.weight", "embeddings.1.weight", "embeddings.2.weight", "embeddings.3.weight",
-                         "_embed.weight", "token.weight", "tokens.weight", "gaussian_matrix")):
-            t = torch.randn(shp, generator=g)
-        else:
-            fan_in = math.prod(shp[1:])
-            if "output_upscaling" in k:                       # ConvTranspose2d weight [in, out, k, k]: fan-in = in
-                fan_in = shp[0]
-            t = torch.randn(shp, generator=g) * fan_in ** -0.5
-        sd[k] = t.to(device, dtype)
+    return {k: _sam_param(k, shp, g).to(device, dtype) for k, shp in shapes.items()}
+
+
+def _sam_param(k, shp, g):
+    """One random SAM parameter (make_sam_state_dict's initialisation rules), drawn from the CPU generator g."""
+    if k.endswith("running_var"):
+        return torch.rand(shp, generator=g) + 0.5
+    if k.endswith("running_mean") or k.endswith(".bias"):
+        return torch.randn(shp, generator=g) * 0.05
+    if len(shp) == 1:                                         # norm gamma
+        return 1.0 + 0.1 * torch.randn(shp, generator=g)
+    if k.endswith(("embeddings.0.weight", "embeddings.1.weight", "embeddings.2.weight", "embeddings.3.weight",
+                   "_embed.weight", "token.weight", "tokens.weight", "gaussian_matrix")):
+        return torch.randn(shp, generator=g)
+    fan_in = math.prod(shp[1:])
+    if "output_upscaling" in k:                               # ConvTranspose2d weight [in, out, k, k]: fan-in = in
+        fan_in = shp[0]
+    return torch.randn(shp, generator=g) * fan_in ** -0.5
+
+
+def make_sam_vit_state_dict(kind: str = "vit_b", seed: int = 0, device="cpu", dtype=torch.float32) -> Dict[str, torch.Tensor]:
+    """A full original-SAM state dict (`image_encoder.*` of ImageEncoderViT [3P] in build_sam's `kind` topology, plus
+    the prompt encoder and mask decoder of make_sam_state_dict) with random weights that keep activations O(1) through
+    the depth: linear weights ~ N(0, 1/fan_in), the two residual branches of each block scaled by depth^-0.5.  The
+    rel-pos tables are NON-zero (SAM initialises them to zero, which would hide a missing bias)."""
+    from .sam_vit import GRID, KINDS, OUT_CHANS, PATCH, WINDOW
+    C, depth, heads, glob = KINDS[kind]
+    hd = C // heads
+    g = torch.Generator(device=device).manual_seed(seed)
+
+    def rn(*shape, scale=1.0):
+        return (torch.randn(*shape, generator=g, device=device) * scale).to(dtype)
+
+    branch = depth ** -0.5
+    p = "image_encoder."
+    sd = {p + "patch_embed.proj.weight": rn(C, 3, PATCH, PATCH, scale=(3 * PATCH * PATCH) ** -0.5),
+          p + "patch_embed.proj.bias": rn(C, scale=0.05), p + "pos_embed": rn(1, GRID, GRID, C, scale=0.1)}
+    for i in range(depth):
+        b = f"{p}blocks.{i}."
+        n = 2 * (GRID if i in glob else WINDOW) - 1
+        for norm in ("norm1", "norm2"):
+            sd[b + norm + ".weight"], sd[b + norm + ".bias"] = 1 + rn(C, scale=0.1), rn(C, scale=0.05)
+        sd[b + "attn.qkv.weight"], sd[b + "attn.qkv.bias"] = rn(3 * C, C, scale=C ** -0.5), rn(3 * C, scale=0.3)
+        sd[b + "attn.proj.weight"], sd[b + "attn.proj.bias"] = rn(C, C, scale=branch * C ** -0.5), rn(C, scale=0.05)
+        sd[b + "attn.rel_pos_h"], sd[b + "attn.rel_pos_w"] = rn(n, hd, scale=0.1), rn(n, hd, scale=0.1)
+        sd[b + "mlp.lin1.weight"], sd[b + "mlp.lin1.bias"] = rn(4 * C, C, scale=C ** -0.5), rn(4 * C, scale=0.05)
+        sd[b + "mlp.lin2.weight"] = rn(C, 4 * C, scale=branch * (4 * C) ** -0.5)
+        sd[b + "mlp.lin2.bias"] = rn(C, scale=0.05)
+    sd[p + "neck.0.weight"] = rn(OUT_CHANS, C, 1, 1, scale=C ** -0.5)
+    sd[p + "neck.2.weight"] = rn(OUT_CHANS, OUT_CHANS, 3, 3, scale=(9 * OUT_CHANS) ** -0.5)
+    for k in ("neck.1", "neck.3"):
+        sd[p + k + ".weight"], sd[p + k + ".bias"] = 1 + rn(OUT_CHANS, scale=0.1), rn(OUT_CHANS, scale=0.05)
+    from oracle.sam_decoder import decoder_shapes
+    gd = torch.Generator().manual_seed(seed + 1)
+    sd.update({k: _sam_param(k, shp, gd).to(device, dtype) for k, shp in decoder_shapes().items()})
     return sd
