@@ -88,11 +88,19 @@ typedef struct {
     const void* col_c1;
     const void* col_c2;
     /* multi-stream launches: streams (row groups) with different LoRA sets have different c1/c2; then col_c1/col_c2
-     * are [n_col_groups][N] and rows [col_group_end[g-1], col_group_end[g]) use plane g (boundaries % 128 == 0). */
+     * are [n_col_groups][N] and rows [col_group_end[g-1], col_group_end[g]) use plane g (boundaries as for
+     * w_group_planes below). */
     int32_t n_col_groups;
     int64_t col_group_end[8];
     int32_t w_group_planes; /* 0: one weight matrix for all rows; else == n_col_groups: w is [planes][N][Ktot] and row
-                             * group g multiplies with plane g (per-stream weights, e.g. W + s B_g A_g merged per concept) */
+                             * group g multiplies with plane g (per-stream weights, e.g. W + s B_g A_g merged per concept).
+                             * Every segment reads plane g (all taps of a conv, the conv2 | shortcut concatenation); bias,
+                             * rowvec, column statistics and the fp32 twins do not depend on the plane.  Not with w2.
+                             * No tile may mix two groups: on a token grid (d.H == 1) every col_group_end is a multiple
+                             * of 128 rows; on a spatial grid (d.H > 1: convs) a tile lies inside one image, so every
+                             * col_group_end is a multiple of d.W * d.H pixels (whole images), whatever the image size.
+                             * Tall tiles pair two consecutive m-tiles; where a boundary would fall inside a pair the
+                             * launch uses single tiles instead. */
     int32_t cta_pair;   /* 0 = auto, 1 = single 128-row tiles, 2 = not available (rejected),
                          * 3 = tall tiles (one CTA, 256 x 160: two 128-row sub-tiles share each weight tile; block_n 160) */
     /* GroupNorm statistics out of the producing GEMM / conv (ResnetBlock2D norm1/norm2, Transformer2DModel.norm,

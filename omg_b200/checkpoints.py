@@ -9,6 +9,10 @@
                                               (also `.lora.down.weight`, `.lora_linear_layer.down.weight`,
                                                `.processor.to_q_lora.down.weight` of older diffusers)
   all become {Linear path: (A [r, in], B [out, r], alpha / r)}; text-encoder entries are returned separately.
+  A LoCon file also wraps the ResBlock convs, time_emb_proj and the down- / up-sampler convs
+  (config.lora_conv_target_names; SGM spellings `input_blocks_4_0_in_layers_2` = conv1, `_emb_layers_1` = time_emb_proj,
+  `_out_layers_3` = conv2, `_skip_connection` = conv_shortcut, `input_blocks_3_0_op`, `output_blocks_2_2_conv`); with
+  conv=True these become {module path: (A [r, in, k, k], B [out, r], alpha / r)}.
 * InstantID `ip-adapter.bin` (instantid_single_pieline.py:179-213): {"image_proj": Resampler state dict,
   "ip_adapter": {"<i>.to_k_ip.weight", "<i>.to_v_ip.weight"}} with i the position of the processor in
   `unet.attn_processors` (registration order: down blocks, up blocks, mid block; attn1 / attn2 alternating).
@@ -21,7 +25,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .config import UNetConfig, lora_target_names, transformer_names
+from .config import UNetConfig, lora_conv_target_names, lora_target_names, transformer_names
 
 LoraDict = Dict[str, Tuple[torch.Tensor, torch.Tensor, float]]
 
@@ -107,6 +111,32 @@ def _kohya_lookup(cfg: UNetConfig) -> Dict[str, str]:
     return table
 
 
+_SGM_RESNET_TAILS = (("in_layers_2", "conv1"), ("emb_layers_1", "time_emb_proj"), ("out_layers_3", "conv2"),
+                     ("skip_connection", "conv_shortcut"))
+
+
+def _kohya_conv_lookup(cfg: UNetConfig) -> Dict[str, str]:
+    """kohya stems (diffusers and SGM block names) of the LoCon modules of lora_conv_target_names."""
+    names = {name for name, _k, _i, _o, _ks in lora_conv_target_names(cfg)}
+    table = {"lora_unet_" + n.replace(".", "_"): n for n in names}
+    lpb, nb = cfg.layers_per_block, len(cfg.block_out_channels)
+    res = {"middle_block_0": "mid_block.resnets.0", "middle_block_2": "mid_block.resnets.1"}
+    for blk in range(nb):
+        for pos in range(lpb):
+            res[f"input_blocks_{1 + blk * (lpb + 1) + pos}_0"] = f"down_blocks.{blk}.resnets.{pos}"
+        for pos in range(lpb + 1):
+            res[f"output_blocks_{blk * (lpb + 1) + pos}_0"] = f"up_blocks.{blk}.resnets.{pos}"
+        if blk < nb - 1:
+            table[f"lora_unet_input_blocks_{(blk + 1) * (lpb + 1)}_0_op"] = f"down_blocks.{blk}.downsamplers.0.conv"
+            sub = 2 if cfg.transformer_layers[nb - 1 - blk] > 0 else 1
+            table[f"lora_unet_output_blocks_{blk * (lpb + 1) + lpb}_{sub}_conv"] = f"up_blocks.{blk}.upsamplers.0.conv"
+    for stem, path in res.items():
+        for tail, leaf in _SGM_RESNET_TAILS:
+            if f"{path}.{leaf}" in names:
+                table[f"lora_unet_{stem}_{tail}"] = f"{path}.{leaf}"
+    return table
+
+
 _PEFT_SUFFIXES = (
     (".lora_A.weight", "A"), (".lora_B.weight", "B"),
     (".lora_A.default.weight", "A"), (".lora_B.default.weight", "B"),
@@ -116,8 +146,13 @@ _PEFT_SUFFIXES = (
 )
 
 
-def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfig] = None, strict: bool = False):
+def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfig] = None, strict: bool = False,
+                            conv: bool = False):
     """-> (unet_lora, text_encoder_lora, skipped).
+
+    conv=True also converts the LoCon modules (ResBlock convs, time_emb_proj, down- / up-sampler convs) to
+    (A [r,in,k,k], B [out,r], alpha/r) - a `lora_up` stored as a 1x1 conv [out,r,1,1] is squeezed - instead of skipping
+    them; what is still skipped then is a module no executor adapts.
 
     unet_lora: {diffusers Linear path: (A [r,in], B [out,r], alpha/r)} for omg_b200 `load_lora_weights`.
     text_encoder_lora: same triple keyed `te1.<path>` / `te2.<path>` (consumed by whoever owns the text encoders).
@@ -126,6 +161,10 @@ def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfi
     cfg = cfg or UNetConfig.sdxl()
     known = {name for name, _i, _o in lora_target_names(cfg)}
     kohya = _kohya_lookup(cfg)
+    convs = {name: (kind, i, o, k) for name, kind, i, o, k in lora_conv_target_names(cfg)} if conv else {}
+    if conv:
+        known |= set(convs)
+        kohya.update(_kohya_conv_lookup(cfg))
     parts: Dict[str, Dict[str, torch.Tensor]] = {}
     te_parts: Dict[str, Dict[str, torch.Tensor]] = {}
     skipped: List[str] = []
@@ -186,7 +225,13 @@ def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfi
             if "A" not in d or "B" not in d:
                 raise ValueError(f"LoRA entry {name} lacks its {'down' if 'A' not in d else 'up'} matrix")
             A, B = d["A"], d["B"]
-            if A.ndim != 2 or B.ndim != 2:
+            if convs.get(name, ("linear",))[0] == "conv":
+                if B.ndim == 4 and tuple(B.shape[2:]) != (1, 1):
+                    raise ValueError(f"LoRA entry {name}: the up kernel is {tuple(B.shape[2:])}, only 1x1 is supported")
+                B = B.flatten(1)
+                if A.ndim == 2:  # Linear spelling of a 1x1 conv
+                    A = A[:, :, None, None]
+            elif A.ndim != 2 or B.ndim != 2:
                 A, B = A.flatten(1), B.flatten(1)  # 1x1-conv spelling of a Linear
             r = A.shape[0]
             if B.shape[1] != r:
@@ -198,17 +243,20 @@ def convert_lora_state_dict(sd: Dict[str, torch.Tensor], cfg: Optional[UNetConfi
     if strict and skipped:
         raise ValueError(f"{len(skipped)} LoRA tensors target modules this path does not adapt, e.g. {skipped[:3]}")
     unet_lora = finish(parts)
-    shapes = {n: (i, o) for n, i, o in lora_target_names(cfg)}
+    shapes = {n: (i, o, 1) for n, i, o in lora_target_names(cfg)}
+    shapes.update({n: (i, o, k) for n, (_kind, i, o, k) in convs.items()})
     for name, (A, B, _s) in unet_lora.items():
-        i, o = shapes[name]
+        i, o, k = shapes[name]
         if A.shape[1] != i or B.shape[0] != o:
             raise ValueError(f"LoRA entry {name}: expected in={i}, out={o}, file has in={A.shape[1]}, out={B.shape[0]}")
+        if A.ndim == 4 and tuple(A.shape[2:]) != (k, k):
+            raise ValueError(f"LoRA entry {name}: expected a {k}x{k} down kernel, file has {tuple(A.shape[2:])}")
     return unet_lora, finish(te_parts), skipped
 
 
-def load_lora(path: str, cfg: Optional[UNetConfig] = None, strict: bool = False):
+def load_lora(path: str, cfg: Optional[UNetConfig] = None, strict: bool = False, conv: bool = False):
     """File -> (unet_lora, text_encoder_lora, skipped); see convert_lora_state_dict."""
-    return convert_lora_state_dict(load_state_dict(path), cfg, strict)
+    return convert_lora_state_dict(load_state_dict(path), cfg, strict, conv)
 
 
 # ------------------------------------------------------------------------------------------------ IP-adapter

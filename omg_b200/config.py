@@ -178,6 +178,25 @@ def lora_target_names(cfg: UNetConfig) -> List[Tuple[str, int, int]]:
     return out
 
 
+def lora_conv_target_names(cfg: UNetConfig) -> List[Tuple[str, str, int, int, int]]:
+    """(module path, kind, in, out, kernel) of the modules a LoCon adapter wraps besides the transformer Linears: every
+    ResnetBlock2D's conv1 / conv2 (3x3), conv_shortcut (1x1, where in != out) and time_emb_proj (kind "linear",
+    kernel 1), the Downsample2D conv (3x3, stride 2) and the Upsample2D conv (3x3 after nearest 2x).  conv_in, conv_out
+    and the embedding MLPs are not LoRA targets (kohya never wraps them)."""
+    out = []
+    for key, shp in param_shapes(cfg).items():
+        if not key.endswith(".weight"):
+            continue
+        name = key[: -len(".weight")]
+        leaf = name.rsplit(".", 1)[-1]
+        if leaf == "time_emb_proj":
+            out.append((name, "linear", shp[1], shp[0], 1))
+        elif (".resnets." in name and leaf in ("conv1", "conv2", "conv_shortcut")) or \
+                name.endswith((".downsamplers.0.conv", ".upsamplers.0.conv")):
+            out.append((name, "conv", shp[1], shp[0], shp[2]))
+    return out
+
+
 def unet_flops(cfg: UNetConfig, H: int, W: int, ctx_len: int = 77, controlnet: bool = False) -> float:
     """Algorithmic FLOPs of one sample-forward at latent H x W: 2*MAC of every conv/linear + 4*N*L*c per
     attention; norms / activations excluded (BASELINE.md section 3)."""

@@ -644,10 +644,21 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     p.w_group_rows = d->w_group_planes > 0 ? d->N : 0;
     OMG_CHECK(d->w_group_planes == 0 || d->w_group_planes == p.n_col_groups, "omg_gemm: w_group_planes must equal n_col_groups");
     OMG_CHECK(p.n_col_groups <= 8, "omg_gemm: at most 8 column-vector row groups");
+    OMG_CHECK(d->w_group_planes == 0 || !d->w2, "omg_gemm: weight planes do not extend to the second weight matrix (w2)");
+    // A tile must not mix two row groups (the producer picks the weight plane, the epilogue the c1 / c2 plane, from the
+    // tile's first pixel).  Token GEMMs (H == 1) walk 128 consecutive rows per tile: boundaries are multiples of 128.
+    // On a spatial grid a tile is a tw x th patch of ONE image, so boundaries are whole numbers of images.
+    const long long img_pix = (long long)W * H;
     for (int i = 0; i < 8; ++i) {
         p.col_group_end[i] = d->col_group_end[i];
-        OMG_CHECK(i + 1 >= p.n_col_groups || d->col_group_end[i] % 128 == 0,
-                  "omg_gemm: row-group boundary %lld is not a multiple of the 128-row tile", (long long)d->col_group_end[i]);
+        if (i + 1 >= p.n_col_groups) continue;
+        if (H > 1)
+            OMG_CHECK(d->col_group_end[i] % img_pix == 0,
+                      "omg_gemm: row-group boundary %lld is inside an image of the %d x %d output grid (boundaries are "
+                      "multiples of %lld pixels)", (long long)d->col_group_end[i], W, H, img_pix);
+        else
+            OMG_CHECK(d->col_group_end[i] % 128 == 0, "omg_gemm: row-group boundary %lld is not a multiple of the 128-row tile",
+                      (long long)d->col_group_end[i]);
     }
     OMG_CHECK(!p.stats_in || (p.col_c1 && p.col_c2 && d->ln_dim > 0 && d->row_stats_parts >= 1 && !d->rowvec),
               "omg_gemm: folded LayerNorm needs col_c1, col_c2, ln_dim, row_stats_parts and no rowvec");
@@ -718,7 +729,9 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     long k_blocks = 0;
     for (int i = 0; i < p.n_segs; ++i) k_blocks += p.segs[i].k_blocks;
     bool pair_ok = true;  // both m-tiles of a tall tile must belong to the same stream
-    for (int i = 0; i + 1 < p.n_col_groups; ++i) pair_ok = pair_ok && (p.col_group_end[i] % 256 == 0);
+    for (int i = 0; i + 1 < p.n_col_groups; ++i)  // spatial grid: the boundary's m-tile index (images x tiles per image) is even
+        pair_ok = pair_ok && (H > 1 ? (p.col_group_end[i] / img_pix * p.tiles_w * p.tiles_h) % 2 == 0
+                                    : p.col_group_end[i] % 256 == 0);
     // tall tiles (256 x 160 per CTA): the narrow-N, long-enough-K GEMMs
     const bool tall = bn == 160 && !geglu && pair_ok &&
                       (d->cta_pair == 3 ||

@@ -191,9 +191,20 @@ def _taps3x3(Cin, a_idx=0, c0=0, k0=0):
     return [(a_idx, kx - 1, ky - 1, c0, Cin, k0 + (ky * 3 + kx) * Cin) for ky in range(3) for kx in range(3)]
 
 
+def _image_groups(row_groups, pixels):
+    """Cumulative image counts of the streams -> group ends in pixels of a launch's output grid (omg_gemm_desc
+    col_group_end: on a spatial grid every boundary is a whole number of images)."""
+    return None if row_groups is None else [e * pixels for e in row_groups]
+
+
 def conv3x3(x, w, bias=None, rowvec=None, residual=None, out=None, shortcut=None, block_n=0, cta_pair=0, colstats=None,
-            residual_f32=None, out_f32=None):
+            residual_f32=None, out_f32=None, row_groups=None):
     """3x3 / stride 1 / pad 1 conv over (B,H,W,Cin).  w = [N, 9*Cin (+ shortcut K)] packed (ky, kx, c).
+
+    row_groups = cumulative image counts [n_1, n_1 + n_2, ..., B] of streams with weights of their own (per-stream LoRA
+    merged into the conv): w is then the stack [len(row_groups) * N, K] and images [n_(g-1), n_g) use plane g.  The same
+    argument of conv3x3_s2 and upsample2x_conv3x3 counts images too; each launch converts it to pixels of ITS output
+    grid (H/2 x W/2 there, the H x W phase grid of the four up-sampler launches).
 
     shortcut = list of (tensor (B,H,W,Ci), weight column offset): 1x1-conv K-segments added to the same accumulator
     (ResnetBlock2D conv_shortcut).  rowvec [B, N] is added per image (time-embedding projection).
@@ -202,6 +213,8 @@ def conv3x3(x, w, bias=None, rowvec=None, residual=None, out=None, shortcut=None
     dt = _op_dtype(x, w, bias, rowvec, residual, out, *[t for t, _ in (shortcut or [])])
     B, H, W, Cin = x.shape
     N, Ktot = w.shape
+    if row_groups is not None:
+        N //= len(row_groups)
     if out is None:
         out = torch.empty((B, H, W, N), dtype=dt, device=x.device)
     views = [view4(x, dt)]
@@ -212,14 +225,18 @@ def conv3x3(x, w, bias=None, rowvec=None, residual=None, out=None, shortcut=None
     gemm(views, segs, w, N, Ktot, view4(out, dt), bias=bias, rowvec=rowvec,
          rowvec_ld=0 if rowvec is None else rowvec.stride(0),
          residual=residual, residual_ld=0 if residual is None else N, block_n=block_n, cta_pair=cta_pair,
-         colstats=None if colstats is None else (colstats, 0), residual_f32=residual_f32, out_f32=out_f32)
+         colstats=None if colstats is None else (colstats, 0), residual_f32=residual_f32, out_f32=out_f32,
+         row_groups=_image_groups(row_groups, H * W))
     return out
 
 
-def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None):
-    """3x3 / stride 2 / pad 1 conv (Downsample2D): A operands are the four stride-2 phase views of x."""
+def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None, row_groups=None):
+    """3x3 / stride 2 / pad 1 conv (Downsample2D): A operands are the four stride-2 phase views of x.
+    row_groups: per-stream weight planes, see conv3x3."""
     B, H, W, Cin = x.shape
     N, Ktot = w.shape
+    if row_groups is not None:
+        N //= len(row_groups)
     assert H % 2 == 0 and W % 2 == 0
     if out is None:
         out = torch.empty((B, H // 2, W // 2, N), dtype=torch.float16, device=x.device)
@@ -231,17 +248,19 @@ def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None):
             px, ox = (1, -1) if kx == 0 else ((0, 0) if kx == 1 else (1, 0))
             segs.append((py * 2 + px, ox, oy, 0, Cin, (ky * 3 + kx) * Cin))
     gemm(views, segs, w, N, Ktot, view4(out), bias=bias, block_n=block_n,
-         colstats=None if colstats is None else (colstats, 0))
+         colstats=None if colstats is None else (colstats, 0), row_groups=_image_groups(row_groups, (H // 2) * (W // 2)))
     return out
 
 
-def upsample2x_conv3x3(x, w, bias=None, out=None, block_n=0, colstats=None):
+def upsample2x_conv3x3(x, w, bias=None, out=None, block_n=0, colstats=None, row_groups=None):
     """nearest-2x upsample followed by 3x3 conv (Upsample2D) without materialising the upsampled tensor:
     each output phase (py,px) is a 9-tap conv over x with shifted taps, stored through a strided output view.
-    fp16 or bf16 (x's type; bf16 without column statistics)."""
+    fp16 or bf16 (x's type; bf16 without column statistics).  row_groups: per-stream weight planes, see conv3x3."""
     dt = _op_dtype(x, w, bias, out)
     B, H, W, Cin = x.shape
     N, Ktot = w.shape
+    if row_groups is not None:
+        N //= len(row_groups)
     if out is None:
         out = torch.empty((B, 2 * H, 2 * W, N), dtype=dt, device=x.device)
     xv = view4(x, dt)
@@ -250,7 +269,8 @@ def upsample2x_conv3x3(x, w, bias=None, out=None, block_n=0, colstats=None):
         for px in range(2):
             segs = [(0, off[px][kx], off[py][ky], 0, Cin, (ky * 3 + kx) * Cin) for ky in range(3) for kx in range(3)]
             cs = None if colstats is None else (colstats, (py * 2 + px) * colstats_blocks(W, H))
-            gemm([xv], segs, w, N, Ktot, view4(out[:, py::2, px::2, :], dt), bias=bias, block_n=block_n, colstats=cs)
+            gemm([xv], segs, w, N, Ktot, view4(out[:, py::2, px::2, :], dt), bias=bias, block_n=block_n, colstats=cs,
+                 row_groups=_image_groups(row_groups, H * W))
     return out
 
 

@@ -17,6 +17,7 @@ UNets (CUDA graphs)] -> omg_fuse_step.  No host sync happens inside the loop.
 """
 import hashlib
 import os
+import sys
 from dataclasses import dataclass
 from typing import Callable, Dict, Optional, Tuple
 
@@ -161,7 +162,10 @@ def _resolve_lora(owner, lora, adapter_name: str, weight_name: Optional[str]):
     path = os.fspath(lora)
     if os.path.isdir(path):
         path = os.path.join(path, weight_name or "pytorch_lora_weights.safetensors")
-    unet_lora, te_lora, skipped = load_lora(path, owner.unet.cfg)
+    unet_lora, te_lora, skipped = load_lora(path, owner.unet.cfg, conv=True)
+    if skipped:
+        print(f"{adapter_name}: {len(skipped)} LoRA tensors of {path} target modules that are not adapted and are "
+              f"ignored, e.g. {skipped[:3]}", file=sys.stderr)
     if not hasattr(owner, "text_encoder_loras"):
         owner.text_encoder_loras = {}
     owner.text_encoder_loras[adapter_name] = te_lora

@@ -6,7 +6,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .config import UNetConfig, lora_target_names, param_shapes
+from .config import UNetConfig, lora_conv_target_names, lora_target_names, param_shapes
 
 
 def make_state_dict(cfg: UNetConfig, seed: int = 0, controlnet: bool = False, device="cpu", dtype=torch.float32,
@@ -35,9 +35,11 @@ def make_state_dict(cfg: UNetConfig, seed: int = 0, controlnet: bool = False, de
 
 
 def make_lora(cfg: UNetConfig, seed: int, rank: int = 32, alpha: Optional[float] = None, device="cpu",
-              dtype=torch.float32) -> Dict[str, Tuple[torch.Tensor, torch.Tensor, float]]:
+              dtype=torch.float32, conv: bool = False) -> Dict[str, Tuple[torch.Tensor, torch.Tensor, float]]:
     """name -> (A [r, in], B [out, r], alpha/r).  Covers every transformer Linear (q,k,v,out,ff.proj,ff.out,
-    proj_in,proj_out)."""
+    proj_in,proj_out).  conv=True (a LoCon adapter) adds the ResBlock / down-sampler / up-sampler modules of
+    lora_conv_target_names with A [r, in, k, k] (A [r, in] for time_emb_proj), drawn from a generator of their own so
+    the Linear entries of a seed are the same either way."""
     g = torch.Generator(device=device).manual_seed(seed)
     alpha = float(rank) if alpha is None else alpha
     out = {}
@@ -45,6 +47,13 @@ def make_lora(cfg: UNetConfig, seed: int, rank: int = 32, alpha: Optional[float]
         A = torch.randn((rank, i), generator=g, device=device) * i ** -0.5
         Bm = torch.randn((o, rank), generator=g, device=device) * rank ** -0.5 * 0.1
         out[name] = (A.to(dtype), Bm.to(dtype), alpha / rank)
+    if conv:
+        gc = torch.Generator(device=device).manual_seed(seed + (1 << 20))
+        for name, kind, i, o, k in lora_conv_target_names(cfg):
+            shape = (rank, i) if kind == "linear" else (rank, i, k, k)
+            A = torch.randn(shape, generator=gc, device=device) * (i * k * k) ** -0.5
+            Bm = torch.randn((o, rank), generator=gc, device=device) * rank ** -0.5 * 0.1
+            out[name] = (A.to(dtype), Bm.to(dtype), alpha / rank)
     return out
 
 

@@ -20,7 +20,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .config import UNetConfig, resnet_names, transformer_names
+from .config import UNetConfig, lora_conv_target_names, lora_target_names, resnet_names, transformer_names
 
 
 def _f16(t, dev):
@@ -47,6 +47,52 @@ CAPTURED_LAUNCHES = [0]
 def total_kernel_launches() -> int:
     """Kernels of this library executed so far: direct launches + launches inside replayed graphs."""
     return L.launch_count() - CAPTURED_LAUNCHES[0] + REPLAYED_LAUNCHES[0]
+
+
+def pack_conv_lora(cfg: UNetConfig, adapters, global_scale: float = 1.0, temb_off: Optional[Dict[str, int]] = None,
+                   device=None) -> Dict[str, List[Tuple[torch.Tensor, torch.Tensor, int, int]]]:
+    """The conv / time-embedding part of a LoRA set (a LoCon adapter: config.lora_conv_target_names), keyed by the
+    packed weight it changes: `<resnet>.w1`, `<resnet>.w2` (conv2 and, behind its 9 * out columns, conv_shortcut),
+    `down<i>.w`, `up<i>.w` and `temb_all.w` (every time_emb_proj, at its rows of the concatenation).
+
+    adapters: list of (lora, adapter_weight), lora[path] = (A [r, in, k, k] | [r, in], B [out, r], alpha / r).
+    Entry: (A [R, K] fp32 in the packed (ky, kx, c) column order, B [n, R] fp32 with  alpha / r * adapter_weight *
+    global_scale  folded in, first row, first column) - the adapters of the set concatenated along R, so that
+    dW[row0 : row0 + n, col0 : col0 + K] = B A  is their sum."""
+    if temb_off is None:
+        temb_off, off = {}, 0
+        for name, cout in resnet_names(cfg):
+            temb_off[name] = off
+            off += cout
+    out: Dict[str, List[Tuple[torch.Tensor, torch.Tensor, int, int]]] = {}
+    for path, kind, _cin, cout, _k in lora_conv_target_names(cfg):
+        As, Bs = [], []
+        for lora, wgt in adapters:
+            if path in lora:
+                A, Bm, s = lora[path]
+                A = A.to(device=device, dtype=torch.float32)
+                As.append(ops.pack_conv3x3_weight(A) if A.dim() == 4 and A.shape[2] == 3 else A.flatten(1))
+                Bs.append(Bm.to(device=device, dtype=torch.float32) * (s * wgt * global_scale))
+        if not As:
+            continue
+        mod, leaf = path.rsplit(".", 1)
+        p = path.split(".")
+        if leaf == "time_emb_proj":
+            key, row0, col0 = "temb_all.w", temb_off[mod], 0
+        elif leaf == "conv":
+            key, row0, col0 = ("down" if p[2] == "downsamplers" else "up") + p[1] + ".w", 0, 0
+        else:
+            key, row0, col0 = mod + (".w1" if leaf == "conv1" else ".w2"), 0, 9 * cout if leaf == "conv_shortcut" else 0
+        out.setdefault(key, []).append((torch.cat(As, dim=0), torch.cat(Bs, dim=1), row0, col0))
+    return out
+
+
+def merge_conv_lora(w: torch.Tensor, entries) -> torch.Tensor:
+    """Packed base weight [N, K] + the deltas of pack_conv_lora entries, summed in fp32 and rounded once."""
+    wf = w.float().clone()
+    for A, Bm, row0, col0 in entries:
+        wf[row0:row0 + Bm.shape[0], col0:col0 + A.shape[1]] += Bm @ A
+    return wf.to(w.dtype)
 
 
 class PackedUNet:
@@ -157,6 +203,8 @@ class PackedUNet:
         # bumped whenever something a captured CUDA graph may have baked in changes (LoRA sets, IP-adapter weights,
         # the IP scale scalar): runners drop their graphs when they see a new version
         self.adapter_version = 0
+        # bumped when a LoRA set is added or replaced: runners drop their merged weight planes
+        self.lora_version = 0
 
     # ------------------------------------------------------------------------------------------- adapters
     def add_lora_set(self, key: str, adapters, global_scale: float = 1.0):
@@ -165,7 +213,9 @@ class PackedUNet:
 
         adapters: list of (lora, adapter_weight); lora maps the diffusers Linear path to (A [r,in], B [out,r],
         alpha/r).  The delta stays un-merged: t = A_cat x is one skinny GEMM, s*B is a second weight matrix whose
-        columns become extra K-segments of the main GEMM."""
+        columns become extra K-segments of the main GEMM.  The conv / time-embedding modules of a LoCon adapter
+        (pack_conv_lora) are kept beside them under the key of the packed weight they change; runners always merge
+        those into per-stream weights."""
         dev = self.device
         packed: Dict[str, Tuple[torch.Tensor, torch.Tensor]] = {}
 
@@ -226,12 +276,15 @@ class PackedUNet:
         known = set()
         for lora, _ in adapters:
             known |= set(lora.keys())
-        from .config import lora_target_names
-        unsupported = known - {n for n, _, _ in lora_target_names(self.cfg)}
+        conv_names = set() if self.controlnet else {t[0] for t in lora_conv_target_names(self.cfg)}
+        unsupported = known - {n for n, _, _ in lora_target_names(self.cfg)} - conv_names
         if unsupported:
-            raise ValueError(f"LoRA targets outside the transformer Linears are not supported: {sorted(unsupported)[:4]}…")
+            raise ValueError("LoRA targets outside the UNet's transformer Linears, ResBlocks and down- / up-samplers are "
+                             f"not supported: {sorted(unsupported)[:4]}…")
+        packed.update(pack_conv_lora(self.cfg, adapters, global_scale, self.temb_off, dev))
         self.lora_sets[key] = packed
         self.adapter_version += 1
+        self.lora_version += 1
 
     def set_ip_adapter(self, ip_weights: Dict[str, Tuple[torch.Tensor, torch.Tensor]], scale: float = 1.0,
                        num_tokens: int = 16):
@@ -292,6 +345,7 @@ class UNetRunner:
         self.warm: set = set()
         self._out: Dict[tuple, object] = {}
         self._graph_version = model.adapter_version
+        self._lora_version = model.lora_version
         self.temb_table = None
         self.kv: Dict[str, torch.Tensor] = {}
         self.kv_ip: Dict[str, torch.Tensor] = {}
@@ -426,6 +480,55 @@ class UNetRunner:
         self._b2_cache[ck] = res
         return res
 
+    def _sync_lora(self):
+        """A LoRA set was added or replaced since the merged weight planes were built: forget them."""
+        if self._lora_version != self.m.lora_version:
+            self._b2_cache.clear()
+            self._lora_version = self.m.lora_version
+
+    def _conv_planes(self, key):
+        """Per-stream weights of the conv (or temb_all) weight `key` for this runner's row groups: None when no group's
+        LoRA set changes it (the launch is then the plain one), else ([G * N, K] fp16 stack - plane g = W + dW_g merged in
+        fp32 and rounded once, the base weight for streams without a delta - and the cumulative image counts)."""
+        sets = self.m.lora_sets
+        if not any(g.lora_key and key in sets[g.lora_key] for g in self.groups):
+            return None
+        ck = "conv|" + key + "|" + ",".join(f"{g.start}-{g.stop}:{g.lora_key}" for g in self.groups)
+        hit = self._b2_cache.get(ck)
+        if hit is None:
+            w = self.m.p[key]
+            planes = [merge_conv_lora(w, sets[g.lora_key][key]) if g.lora_key and key in sets[g.lora_key] else w
+                      for g in self.groups]
+            hit = (torch.cat(planes, dim=0).contiguous(), [g.stop - self.groups[0].start for g in self.groups])
+            self._b2_cache[ck] = hit
+        return hit
+
+    def _conv(self, fn, key, x, shortcut=None, **kw):
+        """fn = ops.conv3x3 | conv3x3_s2 | upsample2x_conv3x3 with the weight `key`.  Streams whose LoRA set has a conv
+        delta for it get their own weight plane in the same launch; where planes are not used (OMG_LORA=unmerged, more
+        than 8 streams) the conv runs once per stream over that stream's images with that stream's merged weight -
+        images are independent in a conv and every other operand is a slice by image."""
+        planes = self._conv_planes(key)
+        if shortcut is not None:
+            kw["shortcut"] = shortcut
+        if planes is None:
+            return fn(x, self.m.p[key], **kw)
+        w, ends = planes
+        if self.merge_lora and len(ends) <= 8:
+            return fn(x, w, row_groups=ends, **kw)
+        B, N = x.shape[0], w.shape[0] // len(ends)
+
+        def rows(t, i0, i1):  # per-image (B, ...) or per-pixel [B * HW, C] operand -> the images [i0, i1)
+            return t[i0 * (t.shape[0] // B):i1 * (t.shape[0] // B)]
+
+        for gi, i1 in enumerate(ends):
+            i0 = ends[gi - 1] if gi else 0
+            kg = {k: (v if k == "bias" or not torch.is_tensor(v) else rows(v, i0, i1)) for k, v in kw.items()}
+            if shortcut is not None:
+                kg["shortcut"] = [(t[i0:i1], off) for t, off in shortcut]
+            fn(x[i0:i1], w[gi * N:(gi + 1) * N], **kg)
+        return kw["out"]
+
     def _lin(self, key, x2d, out, bias=None, residual=None, epilogue=L.EPI_NONE, groups=None, rows_per_item=None,
              stats_out=None, ln=None, colstats=None, residual_f32=None, out_f32=None):
         """Linear with the un-merged LoRA deltas of every row group: t[rows_g, cols_g] = x[rows_g] A_g^T (skinny
@@ -496,7 +599,16 @@ class UNetRunner:
         aug = ops.linear(a, P["add_embedding.linear_2.w"], bias=P["add_embedding.linear_2.b"])
         emb = t_emb.float()[:, None, :] + aug.float()[None, :, :]               # (T, B, 1280)
         act = torch.nn.functional.silu(emb).half().reshape(T * B, -1).contiguous()
+        self._sync_lora()
         self.temb_table = ops.linear(act, P["temb_all.w"], bias=P["temb_all.b"]).reshape(T, B, m.temb_cols)
+        planes = self._conv_planes("temb_all.w")
+        if planes is not None:  # time_emb_proj LoRA: the rows of such a stream come from its merged temb_all plane
+            act3 = act.view(T, B, -1)
+            for gi, g in enumerate(self.groups):
+                if g.lora_key and "temb_all.w" in m.lora_sets[g.lora_key]:
+                    a_g = act3[:, g.start:g.stop].reshape(T * (g.stop - g.start), -1).contiguous()
+                    t_g = ops.linear(a_g, planes[0][gi * m.temb_cols:(gi + 1) * m.temb_cols], bias=P["temb_all.b"])
+                    self.temb_table[:, g.start:g.stop] = t_g.view(T, g.stop - g.start, m.temb_cols)
         self.set_context(ctx, extra_ctx)
 
     def set_context(self, ctx, extra_ctx: Optional[torch.Tensor] = None):
@@ -579,18 +691,18 @@ class UNetRunner:
         a1 = self._gn(x, P[name + ".g1"], P[name + ".b1"], 1e-5, 1, self.buf(name + ".a1", (B, H, W, C1 + C2)), x2=skip)
         off = m.temb_off[name]
         h = self.buf(name + ".h", (B, H, W, cout))
-        ops.conv3x3(a1, P[name + ".w1"], bias=P[name + ".bias1"], rowvec=self.temb_step[:, off:off + cout], out=h,
-                    colstats=self._cs(h, W, H))
+        self._conv(ops.conv3x3, name + ".w1", a1, bias=P[name + ".bias1"], rowvec=self.temb_step[:, off:off + cout], out=h,
+                   colstats=self._cs(h, W, H))
         a2 = self._gn(h, P[name + ".g2"], P[name + ".b2"], 1e-5, 1, self.buf(name + ".a2", (B, H, W, cout)))
         out = self.buf(name + ".out", (B, H, W, cout))
         cs = self._cs(out, W, H)
         if P[name + ".w2"].shape[1] > 9 * cout:
             sc = [(x, 9 * cout)] + ([(skip, 9 * cout + C1)] if skip is not None else [])
-            return ops.conv3x3(a2, P[name + ".w2"], bias=P[name + ".bias2"], shortcut=sc, out=out, colstats=cs,
-                               out_f32=self._twin(out))
+            return self._conv(ops.conv3x3, name + ".w2", a2, bias=P[name + ".bias2"], shortcut=sc, out=out, colstats=cs,
+                              out_f32=self._twin(out))
         r16, r32 = self._res(x)
-        return ops.conv3x3(a2, P[name + ".w2"], bias=P[name + ".bias2"], residual=r16, out=out, colstats=cs,
-                           residual_f32=r32, out_f32=self._twin(out))
+        return self._conv(ops.conv3x3, name + ".w2", a2, bias=P[name + ".bias2"], residual=r16, out=out, colstats=cs,
+                          residual_f32=r32, out_f32=self._twin(out))
 
     def _transformer(self, name, ch, layers, x, variant):
         P, m = self.m.p, self.m
@@ -665,7 +777,7 @@ class UNetRunner:
             if i < nb - 1:
                 B, H, W, _ = h.shape
                 d = self.buf(f"down{i}.out", (B, H // 2, W // 2, ch))
-                h = ops.conv3x3_s2(h, P[f"down{i}.w"], bias=P[f"down{i}.b"], out=d, colstats=self._cs(d, W // 2, H // 2))
+                h = self._conv(ops.conv3x3_s2, f"down{i}.w", h, bias=P[f"down{i}.b"], out=d, colstats=self._cs(d, W // 2, H // 2))
                 skips.append(h)
         ch = cfg.block_out_channels[-1]
         h = self._resblock("mid_block.resnets.0", h)
@@ -708,7 +820,7 @@ class UNetRunner:
             if i < nb - 1:
                 Bh, Hh, Wh, _ = h.shape
                 u = self.buf(f"up{i}.out", (Bh, 2 * Hh, 2 * Wh, ch))
-                h = ops.upsample2x_conv3x3(h, P[f"up{i}.w"], bias=P[f"up{i}.b"], out=u, colstats=self._cs(u, Wh, Hh, launches=4))
+                h = self._conv(ops.upsample2x_conv3x3, f"up{i}.w", h, bias=P[f"up{i}.b"], out=u, colstats=self._cs(u, Wh, Hh, launches=4))
         a = self._gn(h, P["norm_out.g"], P["norm_out.b"], 1e-5, 1, self.buf("norm_out", tuple(h.shape)))
         return ops.conv3x3(a, P["conv_out.w"], bias=P["conv_out.b"], out=self.buf("noise", (B, H, W, 8)))
 
@@ -750,6 +862,7 @@ class UNetRunner:
         """Run one forward for the timestep `step_index` of the schedule given to set_conditioning.  The input is
         whatever self.sample_in holds; returns the (persistent) output buffer(s)."""
         variant = variant or self.default_variant()
+        self._sync_lora()
         self.temb_step.copy_(self.temb_table[step_index])
         fn = self._forward_controlnet if self.m.controlnet else self._forward_unet
         if self.use_plans and key is not None:
