@@ -152,8 +152,8 @@ __global__ void __launch_bounds__(RP_THREADS, 1) attn_relpos_kernel(const __grid
     const int row0 = wg * 64 + wi * 16 + g;  // this thread's rows: row0 and row0 + 8 (accumulator layout, see wgmma.cuh)
     const uint32_t q_addr = smem_u32(q_smem) + wg * (64 * 128);
     const uint32_t q16_addr = smem_u32(q_smem + Lt::Q64) + wg * (64 * 32);
-    mbar_wait(q_full, 0);
-    mbar_wait(t_full, 0);
+    mbar_wait_nocall(q_full, 0);
+    mbar_wait_nocall(t_full, 0);
     // bias tables: Q (64 rows per warpgroup) x table^T in 64-row chunks, scattered by qpos - k + S - 1 = table row
 #pragma unroll 1
     for (int t = 0; t < 2; ++t) {
@@ -211,7 +211,7 @@ __global__ void __launch_bounds__(RP_THREADS, 1) attn_relpos_kernel(const __grid
 
     auto load_kv = [&](int jb) {  // thread 0: block jb into its stage, once both warpgroups have released the stage
         const int st = jb % RP_STAGES;
-        mbar_wait(&kv_empty[st], ((jb / RP_STAGES) & 1) ^ 1);
+        mbar_wait_nocall(&kv_empty[st], ((jb / RP_STAGES) & 1) ^ 1);
         uint8_t* sd = kv_smem + st * Lt::STAGE;
         const int y = y0 + jb * p.byk;
         mbar_arrive_expect_tx(&kv_full[st], 2 * nk_box * D * 2);
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(RP_THREADS, 1) attn_relpos_kernel(const __grid
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, lp[2] = {0.f, 0.f};  // lp: probability mass of padded keys
     for (int j = 0; j < p.nkb; ++j) {
         const int st = j % RP_STAGES;
-        mbar_wait(&kv_full[st], (j / RP_STAGES) & 1);
+        mbar_wait_nocall(&kv_full[st], (j / RP_STAGES) & 1);
         const uint32_t k_addr = smem_u32(kv_smem + st * Lt::STAGE);
         float s[32];
 #pragma unroll

@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_tc_kernel(const __grid_co
     const int kb = p.k_b[item], vb = p.v_b[item];
     auto load_kv = [&](int jb) {  // thread 0: block jb into its stage, once both warpgroups have released the stage
         const int st = jb % ATT_KV_STAGES;
-        mbar_wait(&kv_empty[st], ((jb / ATT_KV_STAGES) & 1) ^ 1);
+        mbar_wait_nocall(&kv_empty[st], ((jb / ATT_KV_STAGES) & 1) ^ 1);
         uint8_t* kd = kv_smem + st * 2 * ATT_K_BYTES;
         mbar_arrive_expect_tx(&kv_full[st], 2 * ATT_K_BYTES);
         tma_load_3d(kd, &p.k_map, &kv_full[st], p.k_col0 + head * ATT_D, jb * ATT_BKV, kb);
@@ -105,10 +105,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_tc_kernel(const __grid_co
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-    mbar_wait(q_full, 0);
+    mbar_wait_nocall(q_full, 0);
     for (int j = 0; j < nkv; ++j) {
         const int st = j % ATT_KV_STAGES;
-        mbar_wait(&kv_full[st], (j / ATT_KV_STAGES) & 1);
+        mbar_wait_nocall(&kv_full[st], (j / ATT_KV_STAGES) & 1);
         const uint32_t k_addr = smem_u32(kv_smem + st * 2 * ATT_K_BYTES);
         float s[32];
 #pragma unroll

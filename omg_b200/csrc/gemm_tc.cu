@@ -8,11 +8,15 @@
 //   A ResBlock's 1x1 shortcut and a LoRA delta  s*B(Ax)  are just more K-segments of the same accumulator.
 // * One CTA per SM, 384 threads: warps 0..7 are two consumer warpgroups (wgmma issue, then the epilogue straight
 //   from the register accumulators), one thread of warpgroup 2 is the TMA producer (setmaxnreg moves that
-//   warpgroup's registers to the consumers: the 128 x 256 accumulator is 128 registers per thread).  The producer runs ahead through a ring of shared-
-//   memory stages, also into the next tile while the consumers are in the epilogue of the current one.
-// * Tile 128 (pixels) x BN (channels) x 64 (K); warpgroup w owns rows 64w..64w+63.  MT = 2 ("tall tile") stacks two
-//   128-row m-tiles that share every weight tile: warpgroup w then owns m-tile w (two m64 blocks).  Operands land in
-//   shared memory in the 128B-swizzled K-major layout the GMMA descriptors expect.
+//   warpgroup's registers to the consumers: a 128 x 160 unit is 160 accumulators per thread).  The producer runs ahead
+//   through a ring of shared-memory stages in the CTA's unit order.
+// * Ping-pong: the work is cut into units of 128 (pixels) x UN (channels, 64 | 128 | 160), K in steps of 64.  Unit j
+//   of a CTA belongs to consumer warpgroup j % 2, which owns it whole (both m64 blocks).  The two warpgroups take turns
+//   on the tensor cores: a warpgroup waits for its turn before its first wgmma of a unit and hands the turn over as
+//   soon as its last wgmma is issued, so one unit's epilogue (and the next unit's per-column vectors) runs while the
+//   other warpgroup's MMAs keep the tensor cores busy.  A logical tile wider than a unit (block_n 256 / 320) runs as
+//   two units of half its width; GEGLU runs on 160-wide units.  Operands land in shared memory in the 128B-swizzled K-major layout the GMMA
+//   descriptors expect.
 //
 // Roofline: tensor-bound; algorithmic FLOPs per launch = 2 * pixels * N * sum(k_len).
 #include <cuda_fp16.h>
@@ -43,7 +47,8 @@ struct alignas(64) GemmParams {
     CUtensorMap b_maps[2];
     SegDev segs[OMG_MAX_SEGS];
     int n_segs;
-    int m_tiles, n_tiles;
+    int units;                 // m_tiles * n_units work units of 128 x UN
+    int n_units;               // units across N: (logical n-tiles) x (units per logical tile)
     int tw, th, tiles_w, tiles_h;
     int img_w, img_h, img_b;
     int N, N_out;
@@ -57,7 +62,8 @@ struct alignas(64) GemmParams {
     int residual_ld;
     int act_silu;
     // LayerNorm folded into the GEMM pair (see omg_gemm_desc): statistics written by the producer's epilogue ...
-    float* stats_out;          // [n_tiles][rows][2] partial (sum, sum of squares) of this GEMM's output rows, or null
+    float* stats_out;          // [planes][rows][2] partial (sum, sum of squares) of this GEMM's output rows, or null
+    int stats_unit_planes;     // k partial planes per unit: unit column nu writes planes nu*k .. nu*k + k-1 (k = 1 for block_n 256)
     // ... and consumed by the next GEMM's epilogue: out = rstd * (acc - mean * c1[n]) + c2[n]
     const float* stats_in;     // [stats_parts][rows][2] or null
     int stats_parts;
@@ -78,26 +84,24 @@ struct alignas(64) GemmParams {
     int cs_rb0, cs_rb_total;
 };
 
-// BN = 320: two N = 160 wgmmas per K step into one 320-column accumulator (wgmma N <= 256).
-// MT = 2: a 256 x BN work unit of two 128-row m-tiles; each consumer warpgroup holds the accumulator of one of them.
+// A unit is 128 rows x UN columns, owned by one consumer warpgroup (two m64 blocks of UN / 2 accumulators each).
 // CS: the epilogue can emit GroupNorm column statistics (FEAT >= 1); only then is their exchange buffer reserved, so the
 // lean instantiations keep that shared memory for pipeline stages.
-template <int BN, int MT, bool CS>
+template <int UN, bool CS>
 struct GemmCfg {
-    static constexpr int WN = BN > 256 ? BN / 2 : BN;  // N of one wgmma
-    static constexpr int NW = BN / WN;                  // wgmmas per m64 block and K = 16 step
-    static constexpr int ACC = MT * BN / 2;             // fp32 accumulators per thread
-    static constexpr int A_BYTES = MT * BM * BK * 2;
-    static constexpr int B_BYTES = BN * BK * 2;
+    static constexpr int ACC = UN;                        // fp32 accumulators per thread
+    static constexpr int A_BYTES = BM * BK * 2;
+    static constexpr int B_BYTES = UN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int VEC_BYTES = 2 * MT * BN * 4;     // per-column epilogue vectors (bias | c1), one plane per m-tile
-    static constexpr int CS_BYTES = CS ? 8 * MT * BN * 8 : 0;  // column-statistics exchange: one float4 per column pair and warp
+    static constexpr int VEC_BYTES = 2 * 2 * UN * 4;      // per warpgroup: the unit's per-column vectors (bias | c1)
+    static constexpr int CS_BYTES = CS ? 2 * 8 * (UN / 2) * 16 : 0;  // per warpgroup: a float4 per column pair and warp of each m64 block
     static constexpr int BARS_BYTES = 256;
     static constexpr int BUDGET = 227 * 1024 - 1024 /*alignment slack*/ - VEC_BYTES - CS_BYTES - BARS_BYTES;
     static constexpr int STAGES_RAW = BUDGET / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
     static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + VEC_BYTES + CS_BYTES + BARS_BYTES;
     static_assert(STAGES >= 2, "shared memory budget");
+    static_assert((2 * STAGES + 2) * 8 <= BARS_BYTES, "barrier space");
 };
 
 // GEGLU / erf-GELU use libdevice's erff.
@@ -108,14 +112,21 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db) {
     if constexpr (std::is_same_v<T, __nv_bfloat16>) {
         if constexpr (WN == 64) wgmma_ss_n64_bf16(*reinterpret_cast<float(*)[32]>(d), da, db, 1u);
         else if constexpr (WN == 128) wgmma_ss_n128_bf16(*reinterpret_cast<float(*)[64]>(d), da, db, 1u);
-        else if constexpr (WN == 160) wgmma_ss_n160_bf16(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
-        else wgmma_ss_n256_bf16(*reinterpret_cast<float(*)[128]>(d), da, db, 1u);
+        else wgmma_ss_n160_bf16(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
     } else {
         if constexpr (WN == 64) wgmma_ss_n64(*reinterpret_cast<float(*)[32]>(d), da, db, 1u);
         else if constexpr (WN == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(d), da, db, 1u);
-        else if constexpr (WN == 160) wgmma_ss_n160(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
-        else wgmma_ss_n256(*reinterpret_cast<float(*)[128]>(d), da, db, 1u);
+        else wgmma_ss_n160(*reinterpret_cast<float(*)[80]>(d), da, db, 1u);
     }
+}
+
+// moves a ring position (stage, phase) on by n k-blocks
+template <int STAGES>
+__device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n) {
+    stage += n;
+    const int wraps = stage / STAGES;
+    stage -= wraps * STAGES;
+    phase ^= (uint32_t)wraps & 1u;
 }
 
 // FEAT selects what the epilogue carries besides bias / time-embedding vector / residual / LayerNorm fold / row statistics:
@@ -125,25 +136,24 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db) {
 //      towers, OMG_TRUNK_F32)
 // T is the storage type of A, W, bias, rowvec, residual and the output (__half, or __nv_bfloat16 for the lean
 // OMG_EPI_NONE instantiations the VAE decoder uses).
-template <typename T, int BN, int EPI, int MT, int FEAT>
+template <typename T, int UN, int EPI, int FEAT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
     using T2 = pair_t<T>;
     constexpr bool kStats = FEAT >= 1, kExtra = FEAT >= 2;
-    static_assert(EPI != OMG_EPI_GEGLU || (BN <= 256 && MT == 1), "GEGLU runs on single 128-row tiles");
-    using Cfg = GemmCfg<BN, MT, kStats>;
+    static_assert(EPI != OMG_EPI_GEGLU || UN == 160, "GEGLU runs on 160-wide units");
+    using Cfg = GemmCfg<UN, kStats>;
     constexpr int STAGES = Cfg::STAGES;
-    constexpr int NJ = BN / 8;  // 8-column chunks of the accumulator
+    constexpr int NJ = UN / 8;  // 8-column chunks of an m64 block's accumulator
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* s_bias = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
-    float* s_c1 = s_bias + MT * BN;
-    float4* s_cs = reinterpret_cast<float4*>(s_c1 + MT * BN);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_cs) + Cfg::CS_BYTES);
+    float* s_vec = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+    float4* s_cs_all = reinterpret_cast<float4*>(s_vec + 2 * 2 * UN);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_cs_all) + Cfg::CS_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
+    uint64_t* turn_bar = empty_bar + STAGES;  // turn_bar[w]: warpgroup w may issue its next unit's wgmmas
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int total_tiles = ((p.m_tiles + MT - 1) / MT) * p.n_tiles;
     const int tiles_per_img = p.tiles_w * p.tiles_h;
 
     if (warp == 8 && lane == 0) {
@@ -152,8 +162,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         tma_prefetch_desc(&p.b_maps[1]);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
+            mbar_init(&empty_bar[i], 1);  // released by the warpgroup that owns the stage's unit
         }
+        mbar_init(&turn_bar[0], 1);
+        mbar_init(&turn_bar[1], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -161,22 +173,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     griddep_wait();               // operands / residual / output buffers belong to earlier kernels until here
 
     if (warp >= 8) {
-        // ------------------------------------------------------------- TMA producer
+        // ------------------------------------------------------------- TMA producer: every unit of the CTA, in order
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 8 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int m_tile = (tile / p.n_tiles) * MT, n_tile = tile % p.n_tiles;
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                const int m_tile = u / p.n_units, nu = u % p.n_units;
                 const int b = m_tile / tiles_per_img;
                 const int rem = m_tile % tiles_per_img;
                 const int h0 = (rem / p.tiles_w) * p.th, w0 = (rem % p.tiles_w) * p.tw;
-                // second 128-row m-tile of a tall tile (the next m-tile in (w, h, image) order; past the last image for
-                // an odd m-tile count: TMA zero-fills)
-                const int b1 = (m_tile + 1) / tiles_per_img, rem1 = (m_tile + 1) % tiles_per_img;
-                const int h1 = (rem1 / p.tiles_w) * p.th, w1 = (rem1 % p.tiles_w) * p.tw;
-                int n0 = n_tile * BN;
-                if (p.w_group_rows > 0) {  // multi-stream launch: this tile's stream selects the weight plane
+                int n0 = nu * UN;
+                if (p.w_group_rows > 0) {  // multi-stream launch: this unit's stream selects the weight plane
                     const long long tile_pix0 = ((long long)b * p.img_h + h0) * p.img_w + w0;
                     for (int g2 = 0; g2 + 1 < p.n_col_groups; ++g2)
                         if (tile_pix0 >= p.col_group_end[g2]) n0 += p.w_group_rows;
@@ -184,18 +192,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 for (int s = 0; s < p.n_segs; ++s) {
                     const SegDev sg = p.segs[s];
                     for (int kb = 0; kb < sg.k_blocks; ++kb) {
-                        mbar_wait(&empty_bar[stage], phase ^ 1);
+                        mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
                         uint8_t* a_dst = smem + stage * Cfg::STAGE_BYTES;
                         uint8_t* b_dst = a_dst + Cfg::A_BYTES;
                         mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
                         tma_load_4d(a_dst, &p.a_maps[sg.a_map], &full_bar[stage], sg.a_c0 + kb * BK, w0 + sg.dx, h0 + sg.dy, b);
-                        if constexpr (MT == 2)
-                            tma_load_4d(a_dst + BM * BK * 2, &p.a_maps[sg.a_map], &full_bar[stage], sg.a_c0 + kb * BK,
-                                        w1 + sg.dx, h1 + sg.dy, b1);
-#pragma unroll
-                        for (int nw = 0; nw < Cfg::NW; ++nw)
-                            tma_load_2d(b_dst + nw * Cfg::WN * BK * 2, &p.b_maps[sg.b_map], &full_bar[stage],
-                                        sg.b_k0 + kb * BK, n0 + nw * Cfg::WN);
+                        tma_load_2d(b_dst, &p.b_maps[sg.b_map], &full_bar[stage], sg.b_k0 + kb * BK, n0);
                         if (++stage == STAGES) {
                             stage = 0;
                             phase ^= 1;
@@ -207,35 +209,44 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         return;
     }
 
-    // ----------------------------------------------------------------- consumer warpgroups
+    // ----------------------------------------------------------------- consumer warpgroups (ping-pong)
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int wg = warp >> 2;         // warpgroup 0 | 1
+    const int wg = warp >> 2;         // warpgroup 0 | 1: units j of the CTA with j % 2 == wg
     const int wi = warp & 3;          // warp within the warpgroup: rows 16 wi .. 16 wi + 15 of each m64 block
     const int g = lane >> 2, c = lane & 3;
-    const int ctid = threadIdx.x;     // 0..255
+    const int wtid = threadIdx.x & 127;
+    float* s_bias = s_vec + wg * (2 * UN);
+    float* s_c1 = s_bias + UN;
+    float4* s_cs = s_cs_all + wg * (8 * (UN / 2));
+    int unit_kb = 0;  // every unit of a launch runs the same K blocks
+    for (int s = 0; s < p.n_segs; ++s) unit_kb += p.segs[s].k_blocks;
     int stage = 0;
     uint32_t phase = 0;
+    if (wg == 1) ring_advance<STAGES>(stage, phase, unit_kb);  // past the CTA's unit 0
+    // warpgroup 0 goes first: parity 1 of a fresh mbarrier reads as a completed phase
+    uint32_t turn_phase = wg == 0 ? 1u : 0u;
     float acc[Cfg::ACC];
 
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int unit_m = (tile / p.n_tiles) * MT, n_tile = tile % p.n_tiles;
-        const int n0 = n_tile * BN;
+    for (int u = blockIdx.x + wg * gridDim.x; u < p.units; u += 2 * gridDim.x) {
+        const int m_tile = u / p.n_units, nu = u % p.n_units;
+        const int n0 = nu * UN;
+        const int b = m_tile / tiles_per_img;
+        const int rem = m_tile % tiles_per_img;
+        const int h0 = (rem / p.tiles_w) * p.th, w0 = (rem % p.tiles_w) * p.tw;
         const bool ln = p.stats_in != nullptr;
 
-        // per-column vectors of every m-tile of the unit (tall tiles: the two m-tiles may belong to different images /
-        // streams); the barrier in front also tells that the previous tile's epilogue is done with them
-        named_bar_sync(1, 256);
-        for (int sub = 0; sub < MT; ++sub) {
-            const int mt = unit_m + sub;
-            const int b = mt / tiles_per_img, rem = mt % tiles_per_img;
-            size_t cg = 0;  // tiles never straddle row groups (host guarantees 128-row alignment): this tile's c1/c2 plane
+        // per-column vectors of the unit, in this warpgroup's own time; the barrier in front also tells that the
+        // previous unit's epilogue is done with them (and with the column-statistics slots)
+        named_bar_sync(1 + wg, 128);
+        {
+            size_t cg = 0;  // units never straddle row groups (host guarantees 128-row alignment): this unit's c1/c2 plane
             if (ln && p.n_col_groups > 1) {
-                const long long tile_pix0 = ((long long)b * p.img_h + (rem / p.tiles_w) * p.th) * p.img_w + (rem % p.tiles_w) * p.tw;
+                const long long tile_pix0 = ((long long)b * p.img_h + h0) * p.img_w + w0;
                 for (int g2 = 0; g2 + 1 < p.n_col_groups; ++g2)
                     if (tile_pix0 >= p.col_group_end[g2]) cg = g2 + 1;
                 cg *= (size_t)p.N;
             }
-            for (int j = ctid; j < BN; j += 256) {
+            for (int j = wtid; j < UN; j += 128) {
                 float v = 0.f, c1 = 0.f;
                 const int n = n0 + j;
                 if (n < p.N) {
@@ -247,38 +258,35 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                         if (p.rowvec && b < p.img_b) v += to_f32(static_cast<const T*>(p.rowvec)[(size_t)b * p.rowvec_ld + n]);
                     }
                 }
-                s_bias[sub * BN + j] = v;
-                s_c1[sub * BN + j] = c1;
+                s_bias[j] = v;
+                s_c1[j] = c1;
             }
         }
-        named_bar_sync(1, 256);
+        named_bar_sync(1 + wg, 128);
 
-        // ------------------------------------------------------------- main loop
+        // ------------------------------------------------------------- main loop, on this warpgroup's turn
 #pragma unroll
         for (int i = 0; i < Cfg::ACC; ++i) acc[i] = 0.f;
+        mbar_wait_nocall(&turn_bar[wg], turn_phase);
+        turn_phase ^= 1;
         int prev_stage = -1;
         for (int s = 0; s < p.n_segs; ++s) {
             const int kbs = p.segs[s].k_blocks;
             for (int kb = 0; kb < kbs; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + (uint32_t)(wg * MT) * (64 * BK * 2);
-                const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+                mbar_wait_nocall(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+                const uint32_t b_addr = a_addr + Cfg::A_BYTES;
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t b_desc = gmma_desc_sw128(b_addr + k * 32, 1024, 16);
 #pragma unroll
-                    for (int i = 0; i < MT; ++i) {
-                        const uint64_t a_desc = gmma_desc_sw128(a_addr + i * (64 * BK * 2) + k * 32, 1024, 16);
-#pragma unroll
-                        for (int nw = 0; nw < Cfg::NW; ++nw) {
-                            const uint64_t b_desc = gmma_desc_sw128(b_addr + nw * (Cfg::WN * BK * 2) + k * 32, 1024, 16);
-                            wgmma_ss<T, Cfg::WN>(acc + i * (BN / 2) + nw * (Cfg::WN / 2), a_desc, b_desc);
-                        }
-                    }
+                    for (int i = 0; i < 2; ++i)
+                        wgmma_ss<T, UN>(acc + i * (UN / 2), gmma_desc_sw128(a_addr + i * (64 * BK * 2) + k * 32, 1024, 16), b_desc);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();  // the previous stage's wgmmas have completed: hand that stage back to the producer
-                if (prev_stage >= 0 && (ctid & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
+                if (prev_stage >= 0 && wtid == 0) mbar_arrive(&empty_bar[prev_stage]);
                 prev_stage = stage;
                 if (++stage == STAGES) {
                     stage = 0;
@@ -286,22 +294,17 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 }
             }
         }
+        // every wgmma of the unit is issued: the other warpgroup's unit may start while these complete
+        if (wtid == 0) mbar_arrive(&turn_bar[wg ^ 1]);
         wgmma_wait<0>();
         reg_fence(acc);
-        if ((ctid & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
+        if (wtid == 0) mbar_arrive(&empty_bar[prev_stage]);
+        ring_advance<STAGES>(stage, phase, unit_kb);  // past the other warpgroup's next unit
 
         // ------------------------------------------------------------- epilogue from the accumulator registers
 #pragma unroll
-        for (int i = 0; i < MT; ++i) {
-            const int blk = wg * MT + i;        // m64 block of the unit
-            const int sub = blk >> 1;           // m-tile of the unit
-            const int m_tile = unit_m + sub;
-            const int b = m_tile / tiles_per_img;
-            const int rem = m_tile % tiles_per_img;
-            const int h0 = (rem / p.tiles_w) * p.th, w0 = (rem % p.tiles_w) * p.tw;
-            const float* sb = s_bias + sub * BN;
-            const float* sc = s_c1 + sub * BN;
-            float* a = acc + i * (BN / 2);
+        for (int blk = 0; blk < 2; ++blk) {  // m64 block of the unit
+            float* a = acc + blk * (UN / 2);
             float row_sum[2] = {0.f, 0.f}, row_sq[2] = {0.f, 0.f};
             bool valid[2];
             size_t pix[2];
@@ -309,7 +312,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
             float ln_a[2] = {1.f, 1.f}, ln_k[2] = {0.f, 0.f};
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int et = (blk & 1) * 64 + wi * 16 + g + 8 * h;  // row of the 128-row m-tile
+                const int et = blk * 64 + wi * 16 + g + 8 * h;  // row of the 128-row m-tile
                 const int ph = h0 + et / p.tw, pw = w0 + et % p.tw;
                 valid[h] = (ph < p.img_h) && (pw < p.img_w) && (b < p.img_b);
                 pix[h] = ((size_t)b * p.img_h + ph) * p.img_w + pw;
@@ -329,10 +332,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 }
             }
             // column statistics: this warp's 16 rows go to its slot of the exchange buffer, (sum, sumsq) per column pair
-            float4* cs_slot = s_cs + (size_t)(blk * 4 + wi) * (BN / 2);
+            float4* cs_slot = s_cs + (size_t)(blk * 4 + wi) * (UN / 2);
 #pragma unroll
             for (int J = 0; J < NJ; ++J) {
-                const int col = 8 * J + 2 * c;  // within the tile
+                const int col = 8 * J + 2 * c;  // within the unit
                 const int n = n0 + col;
                 float x[2][2];
 #pragma unroll
@@ -340,7 +343,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const float v = a[4 * J + 2 * h + e];
-                        x[h][e] = ln ? fmaf(ln_a[h], v, fmaf(ln_k[h], sc[col + e], sb[col + e])) : v + sb[col + e];
+                        x[h][e] = ln ? fmaf(ln_a[h], v, fmaf(ln_k[h], s_c1[col + e], s_bias[col + e])) : v + s_bias[col + e];
                     }
                 if constexpr (EPI == OMG_EPI_GEGLU) {
                     // columns (2i, 2i + 1) are (value, gate) pairs: one output column per pair, two per lane pair
@@ -420,9 +423,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 }
             }
             if constexpr (EPI != OMG_EPI_GEGLU) {
-                if (p.stats_out != nullptr) {  // per-row partials of this tile: the four lanes of a row hold its columns
+                if (p.stats_out != nullptr) {  // per-row partials of this unit: the four lanes of a row hold its columns
                     float2* so = reinterpret_cast<float2*>(p.stats_out);
-                    constexpr int PLANES = BN > 256 ? 4 : 2;  // as many partial planes as two 160-wide tiles would emit
+                    const int kp = p.stats_unit_planes, plane0 = nu * kp;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         float s = row_sum[h], q = row_sq[h];
@@ -431,25 +434,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                         s += __shfl_xor_sync(0xffffffffu, s, 2);
                         q += __shfl_xor_sync(0xffffffffu, q, 2);
                         if (c == 0 && valid[h]) {
-                            so[(size_t)(n_tile * PLANES) * p.stats_rows + pix[h]] = make_float2(s, q);
-                            for (int t = 1; t < PLANES; ++t) so[(size_t)(n_tile * PLANES + t) * p.stats_rows + pix[h]] = make_float2(0.f, 0.f);
+                            so[(size_t)plane0 * p.stats_rows + pix[h]] = make_float2(s, q);
+                            for (int t = 1; t < kp; ++t) so[(size_t)(plane0 + t) * p.stats_rows + pix[h]] = make_float2(0.f, 0.f);
                         }
                     }
                 }
             }
             if constexpr (EPI != OMG_EPI_GEGLU && kStats) {
                 if (p.col_stats != nullptr) {  // the two warps of a 32-row block add their slots
-                    named_bar_sync(2 + wg * 2 + (wi >> 1), 64);
-                    const int q = (blk & 1) * 2 + (wi >> 1);  // 32-row quarter of the m-tile
-                    const float4* s0 = s_cs + (size_t)(blk * 4 + (wi & 2)) * (BN / 2);
-                    const float4* s1 = s0 + BN / 2;
+                    named_bar_sync(3 + wg * 2 + (wi >> 1), 64);
+                    const int q = blk * 2 + (wi >> 1);  // 32-row quarter of the m-tile
+                    const float4* s0 = s_cs + (size_t)(blk * 4 + (wi & 2)) * (UN / 2);
+                    const float4* s1 = s0 + UN / 2;
                     if (b < p.img_b) {
                         const size_t rb = (size_t)b * p.cs_rb_total + p.cs_rb0 + (size_t)rem * 4 + q;
-                        for (int cp = (wi & 1) * 32 + lane; cp < BN / 2; cp += 64) {
+                        for (int cp = (wi & 1) * 32 + lane; cp < UN / 2; cp += 64) {
                             const int col = n0 + 2 * cp;
                             if (col < p.N) {
-                                const float4 u = s0[cp], w = s1[cp];
-                                p.col_stats[(rb * p.N + col) >> 1] = make_float4(u.x + w.x, u.y + w.y, u.z + w.z, u.w + w.w);
+                                const float4 u4 = s0[cp], w4 = s1[cp];
+                                p.col_stats[(rb * p.N + col) >> 1] = make_float4(u4.x + w4.x, u4.y + w4.y, u4.z + w4.z, u4.w + w4.w);
                             }
                         }
                     }
@@ -468,34 +471,33 @@ static int view_to_tmap(CUtensorMap* m, const omg_view4& v, CUtensorMapDataType 
     return make_tmap(m, dt, v.ptr, 4, dims, strides, box, sw);
 }
 
-template <typename T, int BN, int EPI, int MT, int FEAT>
+template <typename T, int UN, int EPI, int FEAT>
 static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, MT, (FEAT >= 1)>;
+    using Cfg = GemmCfg<UN, (FEAT >= 1)>;
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
-        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, BN, EPI, MT, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, UN, EPI, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       Cfg::SMEM_BYTES));
         int dev = 0;
         OMG_CUDA(cudaGetDevice(&dev));
         OMG_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
         configured = true;
     }
-    const int units = ((p.m_tiles + MT - 1) / MT) * p.n_tiles;
-    const int grid = std::min(units, num_sms);
-    OMG_CUDA(launch_pdl(gemm_tc_kernel<T, BN, EPI, MT, FEAT>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
+    const int grid = std::min(p.units, num_sms);
+    OMG_CUDA(launch_pdl(gemm_tc_kernel<T, UN, EPI, FEAT>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
     return check_launch("gemm_tc_kernel");
 }
 
 // FEAT dispatch: 0 lean, 1 + GroupNorm column statistics, 2 + activations / fp32 twins (GEGLU launches are always lean)
-template <int BN, int EPI, int MT = 1>
+template <int UN, int EPI>
 static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
     if constexpr (EPI == OMG_EPI_GEGLU) {
-        return launch_gemm_f<__half, BN, EPI, MT, 0>(p, stream);
+        return launch_gemm_f<__half, UN, EPI, 0>(p, stream);
     } else {
-        if (p.act_silu != 0 || p.residual_f32 != nullptr || p.out_f32 != nullptr) return launch_gemm_f<__half, BN, EPI, MT, 2>(p, stream);
-        if (p.col_stats != nullptr) return launch_gemm_f<__half, BN, EPI, MT, 1>(p, stream);
-        return launch_gemm_f<__half, BN, EPI, MT, 0>(p, stream);
+        if (p.act_silu != 0 || p.residual_f32 != nullptr || p.out_f32 != nullptr) return launch_gemm_f<__half, UN, EPI, 2>(p, stream);
+        if (p.col_stats != nullptr) return launch_gemm_f<__half, UN, EPI, 1>(p, stream);
+        return launch_gemm_f<__half, UN, EPI, 0>(p, stream);
     }
 }
 
@@ -508,32 +510,24 @@ static double tile_time(long tiles, double cols) {
     return (double)((tiles + PLAN_SMS - 1) / PLAN_SMS) * (cols + TILE_OVERHEAD);
 }
 
-// tall tiles (256 x 160): half as many work units, each sharing its weight tiles between two m-tiles
-static bool use_tall_tiles(long m_tiles, long n_tiles, long k_blocks) {
-    if (m_tiles < 2 || k_blocks < 16) return false;
-    return tile_time(((m_tiles + 1) / 2) * n_tiles, 320.0) < tile_time(m_tiles * n_tiles, 160.0);
-}
-
-// k_plan: K blocks the choice is made for; k_blocks: K blocks of this launch.  Row-statistics producers of one consumer
-// must all emit the same number of partials (= 2 * n_tiles), so they - and omg_gemm_plan - choose with k_plan = "long"
-// whatever their own K; whether a 160-wide choice then runs as tall or as 128-row tiles does not change n_tiles.
+// k_plan: K blocks the choice is made for.  Row-statistics producers of one consumer must all emit the same number of
+// partials (= 2 * n_tiles), so they - and omg_gemm_plan - choose with k_plan = "long" whatever their own K.  The fifth
+// candidate prices 160-wide tiles two m-tiles at a time (half the fixed overhead per m-tile) for long enough K.
 constexpr long K_PLAN_LONG = 1000;
-static int pick_block_n(int N, int epilogue, long m_tiles, long k_plan, long k_blocks, bool* prefer_tall) {
-    if (prefer_tall) *prefer_tall = false;
+static int pick_block_n(int N, int epilogue, long m_tiles, long k_plan) {
     if (epilogue == OMG_EPI_GEGLU) return 256;
     const int cands[5] = {256, 160, 128, 64, 160};
     int best = 256;
     double best_t = 1e30;
     for (int i = 0; i < 5; ++i) {
-        const bool tall = i == 4;
-        if (tall && (k_plan < 16 || m_tiles < 2)) continue;
+        const bool pair = i == 4;
+        if (pair && (k_plan < 16 || m_tiles < 2)) continue;
         const long nt = (N + cands[i] - 1) / cands[i];
-        const long mt = tall ? (m_tiles + 1) / 2 : m_tiles;
-        const double t = tile_time(nt * mt, tall ? 2.0 * cands[i] : cands[i]);
+        const long mt = pair ? (m_tiles + 1) / 2 : m_tiles;
+        const double t = tile_time(nt * mt, pair ? 2.0 * cands[i] : cands[i]);
         if (t < best_t - 1e-9) {
             best_t = t;
             best = cands[i];
-            if (prefer_tall) *prefer_tall = tall && k_blocks >= 16;
         }
     }
     return best;
@@ -549,7 +543,7 @@ extern "C" int omg_gemm_plan(int N, int epilogue, int W, int H, int B, int* bloc
     while (tw / 2 >= W && tw > 1) tw /= 2;
     const int th = 128 / tw;
     const long m_tiles = (long)((W + tw - 1) / tw) * ((H + th - 1) / th) * B;
-    const int bn = pick_block_n(N, epilogue, m_tiles, K_PLAN_LONG, 0, nullptr);
+    const int bn = pick_block_n(N, epilogue, m_tiles, K_PLAN_LONG);
     if (block_n) *block_n = bn;
     if (n_tiles) *n_tiles = 2 * ((N + bn - 1) / bn);  // row-statistics partials: one per (n-tile, chunk parity)
     return 0;
@@ -611,21 +605,26 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
     p.img_w = W;
     p.img_h = H;
     p.img_b = B;
-    p.m_tiles = p.tiles_w * p.tiles_h * B;
+    const int m_tiles = p.tiles_w * p.tiles_h * B;
     p.N = d->N;
     p.N_out = N_out;
-    bool prefer_tall = false;
     const long k_blocks_hint = (long)(d->Ktot + (d->w2 ? d->K2tot : 0)) / 64;
     int bn = d->block_n ? d->block_n
-                        : pick_block_n(d->N, d->epilogue, p.m_tiles, d->row_stats_out ? K_PLAN_LONG : k_blocks_hint,
-                                       k_blocks_hint, &prefer_tall);
+                        : pick_block_n(d->N, d->epilogue, m_tiles, d->row_stats_out ? K_PLAN_LONG : k_blocks_hint);
     OMG_CHECK(bn == 64 || bn == 128 || bn == 160 || bn == 256 || bn == 320, "omg_gemm: block_n=%d unsupported", bn);
     OMG_CHECK(bn != 320 || (!geglu && d->N % 320 == 0), "omg_gemm: block_n=320 needs N %% 320 == 0 and no GEGLU");
-    // cta_pair: 0 automatic, 1 single 128-row tiles, 3 tall 256 x 160 tiles; 2 (CTA pairs) has no Hopper counterpart
+    // cta_pair: 0, 1 and 3 (the former tall 256 x 160 tiles) all run the same units; 2 (CTA pairs) has no Hopper counterpart
     OMG_CHECK(d->cta_pair == 0 || d->cta_pair == 1 || d->cta_pair == 3, "omg_gemm: cta_pair=%d unsupported (0, 1 or 3)",
               d->cta_pair);
     if (geglu) bn = 256;
-    p.n_tiles = (d->N + bn - 1) / bn;
+    // a logical tile wider than 160 runs as two units of half its width; each unit writes its share of the tile's
+    // row-statistics partial planes (2 per tile, 4 for block_n 320), so every plane is written exactly once per row
+    // GEGLU (no row statistics, so no planes to share out) runs on the widest unit: more MMA per unit and per staged byte
+    const int unit_n = geglu ? 160 : (bn > 160 ? bn / 2 : bn);
+    const int tile_units = geglu ? 1 : bn / unit_n;
+    p.n_units = geglu ? (d->N + 159) / 160 : (d->N + bn - 1) / bn * tile_units;
+    p.units = m_tiles * p.n_units;
+    p.stats_unit_planes = (bn == 320 ? 4 : 2) / tile_units;
     p.bias = d->bias;
     p.rowvec = d->rowvec;
     p.rowvec_ld = d->rowvec_ld;
@@ -691,7 +690,7 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
         const uint64_t planes = d->w_group_planes > 0 ? (uint64_t)d->w_group_planes : 1;
         const uint64_t dims[2] = {(uint64_t)d->Ktot, (uint64_t)d->N * planes};
         const uint64_t strides[2] = {1, (uint64_t)d->Ktot};
-        const uint32_t box[2] = {BK, (uint32_t)(bn > 256 ? bn / 2 : bn)};
+        const uint32_t box[2] = {BK, (uint32_t)unit_n};
         if (make_tmap(&p.b_maps[0], tdt, d->w, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
         p.b_maps[1] = p.b_maps[0];
     }
@@ -699,7 +698,7 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
         OMG_CHECK(d->K2tot >= 8 && d->K2tot % 8 == 0, "omg_gemm: K2tot=%d must be a positive multiple of 8", d->K2tot);
         const uint64_t dims[2] = {(uint64_t)d->K2tot, (uint64_t)d->N};
         const uint64_t strides[2] = {1, (uint64_t)d->K2tot};
-        const uint32_t box[2] = {BK, (uint32_t)(bn > 256 ? bn / 2 : bn)};
+        const uint32_t box[2] = {BK, (uint32_t)unit_n};
         if (make_tmap(&p.b_maps[1], tdt, d->w2, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
     }
     OMG_CHECK(d->d.sw % 2 == 0 && d->d.sh % 2 == 0 && d->d.sb % 2 == 0 && (reinterpret_cast<uintptr_t>(d->d.ptr) & 3) == 0,
@@ -726,34 +725,18 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
         p.segs[s] = SegDev{sg.a_idx, sg.dx, sg.dy, sg.a_c0, (sg.k_len + BK - 1) / BK, sg.b_k0, sg.b_idx};
     }
 
-    long k_blocks = 0;
-    for (int i = 0; i < p.n_segs; ++i) k_blocks += p.segs[i].k_blocks;
-    bool pair_ok = true;  // both m-tiles of a tall tile must belong to the same stream
-    for (int i = 0; i + 1 < p.n_col_groups; ++i)  // spatial grid: the boundary's m-tile index (images x tiles per image) is even
-        pair_ok = pair_ok && (H > 1 ? (p.col_group_end[i] / img_pix * p.tiles_w * p.tiles_h) % 2 == 0
-                                    : p.col_group_end[i] % 256 == 0);
-    // tall tiles (256 x 160 per CTA): the narrow-N, long-enough-K GEMMs
-    const bool tall = bn == 160 && !geglu && pair_ok &&
-                      (d->cta_pair == 3 ||
-                       (d->cta_pair == 0 && (prefer_tall || use_tall_tiles(p.m_tiles, p.n_tiles, k_blocks))));
-    if (bf16) {  // lean (FEAT 0) OMG_EPI_NONE tiles only: every other feature was rejected above
-        if (tall) return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 2, 0>(p, stream);
-        switch (bn) {
-            case 64: return launch_gemm_f<__nv_bfloat16, 64, OMG_EPI_NONE, 1, 0>(p, stream);
-            case 128: return launch_gemm_f<__nv_bfloat16, 128, OMG_EPI_NONE, 1, 0>(p, stream);
-            case 160: return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 1, 0>(p, stream);
-            case 320: return launch_gemm_f<__nv_bfloat16, 320, OMG_EPI_NONE, 1, 0>(p, stream);
-            default: return launch_gemm_f<__nv_bfloat16, 256, OMG_EPI_NONE, 1, 0>(p, stream);
+    if (bf16) {  // lean (FEAT 0) OMG_EPI_NONE units only: every other feature was rejected above
+        switch (unit_n) {
+            case 64: return launch_gemm_f<__nv_bfloat16, 64, OMG_EPI_NONE, 0>(p, stream);
+            case 128: return launch_gemm_f<__nv_bfloat16, 128, OMG_EPI_NONE, 0>(p, stream);
+            default: return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 0>(p, stream);
         }
     }
-    if (bn == 320) return launch_gemm<320, OMG_EPI_NONE>(p, stream);
-    if (tall) return launch_gemm<160, OMG_EPI_NONE, 2>(p, stream);
-    if (geglu) return launch_gemm<256, OMG_EPI_GEGLU>(p, stream);
-    switch (bn) {
+    if (geglu) return launch_gemm<160, OMG_EPI_GEGLU>(p, stream);
+    switch (unit_n) {
         case 64: return launch_gemm<64, OMG_EPI_NONE>(p, stream);
         case 128: return launch_gemm<128, OMG_EPI_NONE>(p, stream);
-        case 160: return launch_gemm<160, OMG_EPI_NONE>(p, stream);
-        default: return launch_gemm<256, OMG_EPI_NONE>(p, stream);
+        default: return launch_gemm<160, OMG_EPI_NONE>(p, stream);
     }
 }
 

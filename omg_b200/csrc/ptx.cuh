@@ -94,6 +94,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// The same bounded wait without the diagnostic printf, for kernels that keep wgmmas in flight across waits: a function
+// call anywhere in such a kernel makes ptxas serialize its whole wgmma pipeline (C7510, "wgmma pipeline crossing
+// function boundary").
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return;
+    const long long t0 = clock64();
+    uint32_t spins = 0;
+    while (!mbar_try_wait_long(bar, parity))
+        if ((++spins & 0x3FF) == 0 && clock64() - t0 > OMG_MBAR_TIMEOUT_CYCLES) __trap();
+}
+
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
