@@ -14,7 +14,9 @@
 //   of a CTA belongs to consumer warpgroup j % 2, which owns it whole (both m64 blocks).  The two warpgroups take turns
 //   on the tensor cores: a warpgroup waits for its turn before its first wgmma of a unit and hands the turn over as
 //   soon as its last wgmma is issued, so one unit's epilogue (and the next unit's per-column vectors) runs while the
-//   other warpgroup's MMAs keep the tensor cores busy.  A logical tile wider than a unit (block_n 256 / 320) runs as
+//   other warpgroup's MMAs keep the tensor cores busy.  An fp16 residual that a tensor map can describe is staged per
+//   unit in shared memory by a second TMA thread of warpgroup 2, so the epilogue reads it there instead of waiting on
+//   global loads that the aliased output stores keep in order.  A logical tile wider than a unit (block_n 256 / 320) runs as
 //   two units of half its width; GEGLU runs on 160-wide units.  Operands land in shared memory in the 128B-swizzled K-major layout the GMMA
 //   descriptors expect.
 //
@@ -82,12 +84,18 @@ struct alignas(64) GemmParams {
     long long out_f32_ld;
     float4* col_stats;         // GroupNorm statistics of the output: [B][cs_rb_total][N] float2 (sum, sumsq), or null
     int cs_rb0, cs_rb_total;
+    // the residual over the output grid (N, W, H, B), boxes of 32 columns x one tw x th patch, 64B-swizzled (RES kernels)
+    CUtensorMap res_map;
 };
 
 // A unit is 128 rows x UN columns, owned by one consumer warpgroup (two m64 blocks of UN / 2 accumulators each).
 // CS: the epilogue can emit GroupNorm column statistics (FEAT >= 1); only then is their exchange buffer reserved, so the
 // lean instantiations keep that shared memory for pipeline stages.
-template <int UN, bool CS>
+// RES: the residual is staged by TMA into one buffer of UN / 32 boxes of 128 rows x 32 columns, shared by both
+// warpgroups (their epilogues take turns, as their MMAs do).  Stages: 8 / 5 / 5 for UN 64 / 128 / 160 (8 / 5 / 4 with
+// CS), against 8 / 7 / 6 (8 / 6 / 5) without; a buffer per warpgroup would leave 8 / 4 / 3 (7 / 4 / 3).
+constexpr int RES_BOX_BYTES = BM * 32 * 2;
+template <int UN, bool CS, bool RES = false>
 struct GemmCfg {
     static constexpr int ACC = UN;                        // fp32 accumulators per thread
     static constexpr int A_BYTES = BM * BK * 2;
@@ -95,13 +103,15 @@ struct GemmCfg {
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int VEC_BYTES = 2 * 2 * UN * 4;      // per warpgroup: the unit's per-column vectors (bias | c1)
     static constexpr int CS_BYTES = CS ? 2 * 8 * (UN / 2) * 16 : 0;  // per warpgroup: a float4 per column pair and warp of each m64 block
+    static constexpr int RES_BYTES = RES ? (UN / 32) * RES_BOX_BYTES : 0;
     static constexpr int BARS_BYTES = 256;
-    static constexpr int BUDGET = 227 * 1024 - 1024 /*alignment slack*/ - VEC_BYTES - CS_BYTES - BARS_BYTES;
+    static constexpr int BUDGET = 227 * 1024 - 1024 /*alignment slack*/ - RES_BYTES - VEC_BYTES - CS_BYTES - BARS_BYTES;
     static constexpr int STAGES_RAW = BUDGET / STAGE_BYTES;
     static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + VEC_BYTES + CS_BYTES + BARS_BYTES;
+    static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + RES_BYTES + VEC_BYTES + CS_BYTES + BARS_BYTES;
     static_assert(STAGES >= 2, "shared memory budget");
-    static_assert((2 * STAGES + 2) * 8 <= BARS_BYTES, "barrier space");
+    static_assert(STAGE_BYTES % 1024 == 0, "the residual buffer follows the stages on a 1024 B boundary");
+    static_assert((2 * STAGES + 5) * 8 <= BARS_BYTES, "barrier space");
 };
 
 // GEGLU / erf-GELU use libdevice's erff.
@@ -136,21 +146,28 @@ __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n)
 //      towers, OMG_TRUNK_F32)
 // T is the storage type of A, W, bias, rowvec, residual and the output (__half, or __nv_bfloat16 for the lean
 // OMG_EPI_NONE instantiations the VAE decoder uses).
-template <typename T, int UN, int EPI, int FEAT>
+// RES (fp16, FEAT 0 / 1): the residual comes from shared memory, staged per unit by a second TMA thread, instead of one
+// dependent global load per 8-column chunk in the epilogue (the output may alias the residual, so those loads cannot be
+// hoisted above the stores).
+template <typename T, int UN, int EPI, int FEAT, bool RES = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
     using T2 = pair_t<T>;
     constexpr bool kStats = FEAT >= 1, kExtra = FEAT >= 2;
     static_assert(EPI != OMG_EPI_GEGLU || UN == 160, "GEGLU runs on 160-wide units");
-    using Cfg = GemmCfg<UN, kStats>;
+    static_assert(!RES || (std::is_same_v<T, __half> && EPI == OMG_EPI_NONE && FEAT <= 1), "staged residual: fp16, FEAT 0 / 1");
+    using Cfg = GemmCfg<UN, kStats, RES>;
     constexpr int STAGES = Cfg::STAGES;
     constexpr int NJ = UN / 8;  // 8-column chunks of an m64 block's accumulator
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    float* s_vec = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint8_t* s_res = smem + STAGES * Cfg::STAGE_BYTES;
+    float* s_vec = reinterpret_cast<float*>(s_res + Cfg::RES_BYTES);
     float4* s_cs_all = reinterpret_cast<float4*>(s_vec + 2 * 2 * UN);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_cs_all) + Cfg::CS_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* turn_bar = empty_bar + STAGES;  // turn_bar[w]: warpgroup w may issue its next unit's wgmmas
+    uint64_t* res_full = turn_bar + 2;        // res_full[w]: the residual of warpgroup w's next unit has landed
+    uint64_t* res_empty = res_full + 2;       // the owner of the buffered residual has read it (one arrival per warp)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -166,6 +183,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         }
         mbar_init(&turn_bar[0], 1);
         mbar_init(&turn_bar[1], 1);
+        if constexpr (RES) {
+            tma_prefetch_desc(&p.res_map);
+            mbar_init(&res_full[0], 1);
+            mbar_init(&res_full[1], 1);
+            mbar_init(res_empty, 4);
+        }
         fence_barrier_init();
     }
     __syncthreads();
@@ -203,6 +226,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                             phase ^= 1;
                         }
                     }
+                }
+            }
+        }
+        if constexpr (RES) {
+            // residual producer: the same units in the same order, one at a time through the shared buffer.  A thread of
+            // its own, so that waiting for the buffer never holds up the operand ring.  The residual's columns are the
+            // output's (no weight-plane offset).
+            if (warp == 9 && lane == 0) {
+                int j = 0;  // unit of the CTA: warpgroup j % 2 reads it
+                for (int u = blockIdx.x; u < p.units; u += gridDim.x, ++j) {
+                    const int m_tile = u / p.n_units, nu = u % p.n_units;
+                    const int b = m_tile / tiles_per_img;
+                    const int rem = m_tile % tiles_per_img;
+                    const int h0 = (rem / p.tiles_w) * p.th, w0 = (rem % p.tiles_w) * p.tw;
+                    mbar_wait_nocall(res_empty, (j & 1) ^ 1);  // unit j - 1's epilogue has read the buffer
+                    mbar_arrive_expect_tx(&res_full[j & 1], Cfg::RES_BYTES);
+#pragma unroll
+                    for (int i = 0; i < UN / 32; ++i)
+                        tma_load_4d(s_res + i * RES_BOX_BYTES, &p.res_map, &res_full[j & 1], nu * UN + 32 * i, w0, h0, b);
                 }
             }
         }
@@ -302,6 +344,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         ring_advance<STAGES>(stage, phase, unit_kb);  // past the other warpgroup's next unit
 
         // ------------------------------------------------------------- epilogue from the accumulator registers
+        // staged residual of row et = blk * 64 + wi * 16 + g + 8 h, columns 8 J + 2 c, 2 c + 1: box J / 4, 64-byte row et,
+        // 16-byte chunk J % 4 under the 64B swizzle (chunk ^= (et >> 1) & 3 = g >> 1, as et - g is a multiple of 8).  A
+        // warp's read of one (J, h) falls on 32-bit bank 16 (g & 1) + 4 ((J % 4) ^ (g >> 1)) + c: a different bank per lane.
+        // (s_res is 1024 B aligned and bits 4, 5 of (wi * 16 + g) * 64 + 4 c are clear, so the chunk is XORed into them)
+        const uint32_t res_row = (smem_u32(s_res) + (wi * 16 + g) * 64 + 4 * c) | ((g >> 1) << 4);
+        if constexpr (RES) mbar_wait_nocall(&res_full[wg], turn_phase ^ wg);  // this warpgroup's k-th unit: parity k % 2
 #pragma unroll
         for (int blk = 0; blk < 2; ++blk) {  // m64 block of the unit
             float* a = acc + blk * (UN / 2);
@@ -380,7 +428,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const bool ok = valid[h] && n < p.N;
-                        if (ok && p.residual != nullptr) {
+                        if constexpr (RES) {
+                            const uint32_t rb = ld_shared_b32((res_row ^ ((J & 3) << 4)) + (J >> 2) * RES_BOX_BYTES + blk * 64 * 64 + h * 8 * 64);
+                            const T2 rv = *reinterpret_cast<const T2*>(&rb);
+                            if (ok) {
+                                const float2 r = to_f32x2(rv);
+                                x[h][0] += r.x;
+                                x[h][1] += r.y;
+                            }
+                        } else if (ok && p.residual != nullptr) {
                             const float2 r = to_f32x2(*reinterpret_cast<const T2*>(static_cast<const T*>(p.residual) + pix[h] * (size_t)p.residual_ld + n));
                             x[h][0] += r.x;
                             x[h][1] += r.y;
@@ -420,6 +476,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                             if (g == 0) cs_slot[4 * J + c] = cs;
                         }
                     }
+                }
+            }
+            if constexpr (RES) {
+                if (blk == 1) {  // the last read of the buffer: the residual thread may refill it for the next unit
+                    __syncwarp();
+                    if (elect_one()) mbar_arrive(res_empty);
                 }
             }
             if constexpr (EPI != OMG_EPI_GEGLU) {
@@ -471,13 +533,13 @@ static int view_to_tmap(CUtensorMap* m, const omg_view4& v, CUtensorMapDataType 
     return make_tmap(m, dt, v.ptr, 4, dims, strides, box, sw);
 }
 
-template <typename T, int UN, int EPI, int FEAT>
+template <typename T, int UN, int EPI, int FEAT, bool RES = false>
 static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
-    using Cfg = GemmCfg<UN, (FEAT >= 1)>;
+    using Cfg = GemmCfg<UN, (FEAT >= 1), RES>;
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
-        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, UN, EPI, FEAT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        OMG_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, UN, EPI, FEAT, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       Cfg::SMEM_BYTES));
         int dev = 0;
         OMG_CUDA(cudaGetDevice(&dev));
@@ -485,19 +547,21 @@ static int launch_gemm_f(const GemmParams& p, cudaStream_t stream) {
         configured = true;
     }
     const int grid = std::min(p.units, num_sms);
-    OMG_CUDA(launch_pdl(gemm_tc_kernel<T, UN, EPI, FEAT>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
+    OMG_CUDA(launch_pdl(gemm_tc_kernel<T, UN, EPI, FEAT, RES>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p));
     return check_launch("gemm_tc_kernel");
 }
 
-// FEAT dispatch: 0 lean, 1 + GroupNorm column statistics, 2 + activations / fp32 twins (GEGLU launches are always lean)
+// FEAT dispatch: 0 lean, 1 + GroupNorm column statistics, 2 + activations / fp32 twins (GEGLU launches are always lean).
+// res_staged: p.res_map describes the residual, so FEAT 0 / 1 launches stage it by TMA.
 template <int UN, int EPI>
-static int launch_gemm(const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const GemmParams& p, bool res_staged, cudaStream_t stream) {
     if constexpr (EPI == OMG_EPI_GEGLU) {
         return launch_gemm_f<__half, UN, EPI, 0>(p, stream);
     } else {
         if (p.act_silu != 0 || p.residual_f32 != nullptr || p.out_f32 != nullptr) return launch_gemm_f<__half, UN, EPI, 2>(p, stream);
-        if (p.col_stats != nullptr) return launch_gemm_f<__half, UN, EPI, 1>(p, stream);
-        return launch_gemm_f<__half, UN, EPI, 0>(p, stream);
+        if (p.col_stats != nullptr)
+            return res_staged ? launch_gemm_f<__half, UN, EPI, 1, true>(p, stream) : launch_gemm_f<__half, UN, EPI, 1>(p, stream);
+        return res_staged ? launch_gemm_f<__half, UN, EPI, 0, true>(p, stream) : launch_gemm_f<__half, UN, EPI, 0>(p, stream);
     }
 }
 
@@ -732,11 +796,22 @@ static int gemm_impl(const omg_gemm_desc* d, void* stream_) {
             default: return launch_gemm_f<__nv_bfloat16, 160, OMG_EPI_NONE, 0>(p, stream);
         }
     }
-    if (geglu) return launch_gemm<160, OMG_EPI_GEGLU>(p, stream);
+    if (geglu) return launch_gemm<160, OMG_EPI_GEGLU>(p, false, stream);
+    // The residual is staged by TMA when a tensor map can describe it: 16 B aligned base (ld % 8 == 0 is checked above).
+    // Otherwise the epilogue reads it from global memory as before.  Boxes clip at N and at the grid's edges, so columns
+    // past N and pixels outside the image are zero-filled, never read.
+    bool res_staged = false;
+    if (d->residual != nullptr && (reinterpret_cast<uintptr_t>(d->residual) & 15) == 0) {
+        const uint64_t ld = (uint64_t)d->residual_ld;
+        const uint64_t dims[4] = {(uint64_t)N_out, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+        const uint64_t strides[4] = {1, ld, ld * W, ld * W * H};
+        const uint32_t box[4] = {32, (uint32_t)tw, (uint32_t)th, 1};
+        res_staged = make_tmap(&p.res_map, tdt, d->residual, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B) == 0;
+    }
     switch (unit_n) {
-        case 64: return launch_gemm<64, OMG_EPI_NONE>(p, stream);
-        case 128: return launch_gemm<128, OMG_EPI_NONE>(p, stream);
-        default: return launch_gemm<160, OMG_EPI_NONE>(p, stream);
+        case 64: return launch_gemm<64, OMG_EPI_NONE>(p, res_staged, stream);
+        case 128: return launch_gemm<128, OMG_EPI_NONE>(p, res_staged, stream);
+        default: return launch_gemm<160, OMG_EPI_NONE>(p, res_staged, stream);
     }
 }
 

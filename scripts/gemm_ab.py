@@ -7,7 +7,9 @@ A/B of library builds.
                                                    print per shape the median and spread over rounds of every build
 
 Every launch uses the automatic tile choice and the epilogue the UNet uses (GEGLU for ff1, a residual for attn-out / ff2);
-a timed launch is the median of 20 CUDA-event-timed launches with L2 flushed before each.  One JSON line per shape."""
+each residual shape also runs as the transformer blocks run it - in place (out = residual) with row statistics out
+(`_inplace`) - and with the same row statistics but no residual (`_plain`), so the residual's own cost is the gap
+between those two rows.  A timed launch is the median of 20 CUDA-event-timed launches with L2 flushed before each.  One JSON line per shape."""
 import argparse
 import json
 import os
@@ -63,7 +65,15 @@ def measure():
             out = torch.empty(M, N // 2 if kind == "geglu" else N, device=dev, dtype=torch.float16)
             epi = L.EPI_GEGLU if kind == "geglu" else L.EPI_NONE
             ms = timeit(lambda: ops.linear(x, w, residual=res, out=out, epilogue=epi))
-            rows.append({"name": f"{tag}_b{batch}", "M": M, "N": N, "K": K, "gflop": 2.0 * M * N * K / 1e9, "us": ms * 1e3})
+            row = {"M": M, "N": N, "K": K, "gflop": 2.0 * M * N * K / 1e9}
+            rows.append({"name": f"{tag}_b{batch}", **row, "us": ms * 1e3})
+            if kind == "residual":
+                stats = torch.empty(ops.gemm_plan(N, L.EPI_NONE, M)[1], M, 2, device=dev)
+                ms = timeit(lambda: ops.linear(x, w, residual=out, out=out, stats_out=stats))
+                rows.append({"name": f"{tag}_inplace_b{batch}", **row, "us": ms * 1e3})
+                ms = timeit(lambda: ops.linear(x, w, out=out, stats_out=stats))
+                rows.append({"name": f"{tag}_plain_b{batch}", **row, "us": ms * 1e3})
+                del stats
             del x, w, res, out
         for tag, H, Cin, N in CONVS:
             x = rnd(batch, H, H, Cin)
