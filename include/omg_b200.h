@@ -325,6 +325,54 @@ typedef struct {
 
 int omg_attention_relpos(const omg_attn_relpos_desc* desc, void* stream);
 
+/*
+ * Face analysis (insightface FaceAnalysis('antelopev2'): an SCRFD detector and an ArcFace IResNet recogniser).  Their
+ * convolutions and the recogniser's FC run on omg_gemm; these are the ops that are not GEMM-shaped.
+ *
+ * omg_channel_op: channels-last fp16, fp32 arithmetic, over B x H x W pixels of C channels (x / y rows of ldx / ldy
+ *   elements):  v = x[p, c] * scale[c] + shift[c];  y[p, c] = act(v) + a  (act_after_add = 0) or act(v + a) (= 1), where
+ *   a = addend[b, y / add_scale, x / add_scale, c] (rows of ld_add elements, grid H / add_scale x W / add_scale: the
+ *   nearest x2 up-sampling of an FPN top-down path when add_scale = 2) or 0 without an addend (add_scale 0).  x may be
+ *   NULL (read as 0: a nearest up-sampling on its own), scale / shift NULL (1 / 0).  act: OMG_CH_ACT_*; PReLU reads
+ *   slope[c].  scale, shift and slope are fp32 [C].  y may alias x; it must not overlap the addend.
+ * omg_pool2d: max (is_max = 1) or average pooling, k x k window (1 <= k <= 3), stride 1 | 2, symmetric pad < k, with
+ *   ONNX / PyTorch ceil_mode and count_include_pad.  x [B, H, W, C] and y [B, Ho, Wo, C] contiguous, C % 8 == 0.
+ * omg_scrfd_detect: SCRFD.detect after the network, in one CTA: anchors with score >= det_thresh (strides' row-major
+ *   grids, num_anchors consecutive anchors per cell, centre (x, y) * stride), distance2bbox / distance2kps of the
+ *   predictions times the stride, / det_scale, a descending sort of the scores (ties: lower anchor index first) and
+ *   greedy NMS with the +1 pixel area convention (suppress when IoU > nms_thresh), all in fp32 with no contraction.
+ *   Writes rows [x1, y1, x2, y2, score, kx0, ky0, .., kx4, ky4] to out (fp32, capacity max_out rows) and the row count
+ *   to *count (device int).  Every anchor of the levels must fit the CTA's shared memory (13 B each, at most
+ *   OMG_SCRFD_MAX_ANCHORS: 640 x 640 with strides 8 / 16 / 32 and two anchors is 16 800); max_out must be at least the
+ *   number of anchors, so no face can be dropped.
+ */
+#define OMG_CH_ACT_NONE 0
+#define OMG_CH_ACT_RELU 1
+#define OMG_CH_ACT_PRELU 2
+#define OMG_CH_ACT_SIGMOID 3
+int omg_channel_op(const void* x, long long ldx, void* y, long long ldy, const float* scale, const float* shift,
+                   const float* slope, const void* addend, long long ld_add, int add_scale, int B, int H, int W, int C,
+                   int act, int act_after_add, void* stream);
+int omg_pool2d(const void* x, void* y, int B, int H, int W, int C, int k, int stride, int pad, int ceil_mode,
+               int count_include_pad, int is_max, void* stream);
+
+#define OMG_SCRFD_MAX_LEVELS 5
+#define OMG_SCRFD_MAX_ANCHORS 17800
+typedef struct {
+    const float* scores[OMG_SCRFD_MAX_LEVELS];  /* [fh * fw * num_anchors] per level */
+    const float* boxes[OMG_SCRFD_MAX_LEVELS];   /* [fh * fw * num_anchors, 4] distances in units of the stride */
+    const float* kps[OMG_SCRFD_MAX_LEVELS];     /* [fh * fw * num_anchors, 10], or NULL everywhere (no key-points) */
+    int32_t stride[OMG_SCRFD_MAX_LEVELS];
+    int32_t fh[OMG_SCRFD_MAX_LEVELS], fw[OMG_SCRFD_MAX_LEVELS];
+    int32_t n_levels, num_anchors;
+    float det_thresh, nms_thresh, det_scale;
+    float* out;       /* [max_out, 15] */
+    int32_t max_out;
+    int32_t* count;   /* device */
+} omg_scrfd_desc;
+
+int omg_scrfd_detect(const omg_scrfd_desc* desc, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Launch plans: a forward as a handle.  The reference drives one UNet forward as a Python call
  * (`self.unet(latent_model_input, t, ...)`, src/pipelines/lora_pipeline.py:558-567, 588-606); a host that is not Python -

@@ -4,11 +4,16 @@ inference_instantid.py:259-286, pinned by tests/golden/cli_flags.json), prompt m
 files; additions (non-breaking): --synthetic, --tiny, --num_inference_steps, --image_size, --dedup, --mask_boxes,
 --face_embeds, --face_kps, --sam_boxes, --decode.
 
-Face analysis (insightface antelopev2) and detection sit outside the accelerated hot path (SURVEY section 8): when
-`insightface` is not importable the identities come from --face_embeds (one 512-d .pt / .npy per region) and the
-stage-2 key-points from --face_kps; regions come from --mask_boxes or --sam_boxes.  In --synthetic mode identities are
-unit-norm random 512-d embeddings (seeds 1, 2), the IdentityNet condition is the reference's `draw_kps_multi` rendering
-of fixed key-points and the masks are the config rectangles.
+Face analysis: insightface's FaceAnalysis('antelopev2') when `insightface` is importable; otherwise, when
+<antelopev2_path>/models/antelopev2/ holds scrfd_10g_bnkps.onnx and glintr100.onnx, omg_b200.face.FaceAnalysis runs the
+two models on the kernels (no real antelopev2 file has been run through it yet).  The face analyser gives the identity
+embeddings of the reference photos and, with a decoded stage-1 image, the key-points of its faces for the stage-2
+IdentityNet condition (`draw_kps_multi`), as the reference does; --face_embeds (one 512-d .pt / .npy per region) and
+--face_kps override either.  Key-points detected on the stage-1 image are also written to face_kps.json with the
+condition image stage-2-condition.png.  Regions come from --mask_boxes or --sam_boxes.  In --synthetic mode identities
+are unit-norm random 512-d embeddings (seeds 1, 2), the IdentityNet condition is the reference's `draw_kps_multi`
+rendering of fixed key-points and the masks are the config rectangles - unless the antelopev2 folder holds the two
+model files, which are then used the same way.
 
 Output: with --decode the VAE decodes both stages to stage-1.png / stage-2.png as the reference writes them - the
 checkpoint's own VAE (<pretrained_model>/vae) in bf16, whose exponent range holds activations that overflow fp16 with
@@ -142,8 +147,21 @@ def build_model_sd(pretrained_model, controlnet_path, face_adapter, device, prom
                            providers=["CUDAExecutionProvider", "CPUExecutionProvider"])
         app.prepare(ctx_id=0, det_size=(640, 640))
     except ImportError:
-        print("insightface not importable: identities from --face_embeds, key-points from --face_kps")
+        app = kernel_face_app(antelopev2_path)
+        if app is None:
+            print("insightface not importable: identities from --face_embeds, key-points from --face_kps")
     return pipe, controller, pipe_concept, app
+
+
+def kernel_face_app(antelopev2_path):
+    """omg_b200.face.FaceAnalysis over <antelopev2_path>/models/antelopev2, or None when its two model files are absent."""
+    from omg_b200 import face
+    if face.antelopev2_files(antelopev2_path) is None:
+        return None
+    app = face.FaceAnalysis(name="antelopev2", root=antelopev2_path)
+    app.prepare(ctx_id=0, det_size=(640, 640))
+    print(f"face analysis on the kernels: {antelopev2_path}/models/antelopev2")
+    return app
 
 
 def _load_vec(path):
@@ -233,6 +251,12 @@ if __name__ == "__main__":
         kps = [[[300 * s + dx * s, 380 * s], [400 * s + dx * s, 380 * s], [350 * s + dx * s, 440 * s],
                 [310 * s + dx * s, 500 * s], [390 * s + dx * s, 500 * s]] for dx in (0, 380)][: len(regions)]
         masks = synthetic.rect_masks(len(regions), (size, size))
+        face_app = kernel_face_app(args.antelopev2_path)
+        if face_app is not None:   # identities from the reference photos, key-points from the stage-1 image
+            faces, kps = [_load_vec(f) for f in args.face_embeds.split("|") if f] or None, None
+            if args.face_kps:
+                import json
+                kps = json.load(open(args.face_kps))
     else:
         pipe, controller, cm, face_app = build_model_sd(args.pretrained_model, args.controlnet_path,
                                                         args.face_adapter_path, device, list(prompts), args.antelopev2_path,
@@ -289,6 +313,19 @@ if __name__ == "__main__":
         for k, m in enumerate(masks):
             print(f"SAM mask {k}: " + ("no box, region skipped" if m is None else f"{int(m.sum())} pixels"))
     if any(m is not None for m in masks):
+        if kps is None and face_app is not None and decoded:
+            # the key-points of the faces in the stage-1 image (inference_instantid.py:352-354)
+            import cv2
+            import json
+            from PIL import Image
+            kps = [np.asarray(f["kps"]).tolist() for f in
+                   face_app.get(cv2.cvtColor(np.array(image[0]), cv2.COLOR_RGB2BGR))]
+            print(f"stage-1 image: {len(kps)} faces")
+            kps_dir = os.path.join(args.save_dir, f"seed_{args.seed}")
+            os.makedirs(kps_dir, exist_ok=True)
+            with open(os.path.join(kps_dir, "face_kps.json"), "w") as fk:
+                json.dump(kps, fk)
+            Image.fromarray(draw_kps_multi((width, height), kps)).save(os.path.join(kps_dir, "stage-2-condition.png"))
         if kps is None:
             raise SystemExit("stage 2 needs the faces' key-points: --face_kps (insightface on the decoded stage-1 image "
                              "is outside the path)")

@@ -60,6 +60,20 @@ class AttnRelposDesc(C.Structure):
                 ("k_bias", C.c_void_p), ("v_bias", C.c_void_p), ("scale", C.c_float)]
 
 
+OMG_SCRFD_MAX_LEVELS = 5
+OMG_SCRFD_MAX_ANCHORS = 17800
+CH_ACT_NONE, CH_ACT_RELU, CH_ACT_PRELU, CH_ACT_SIGMOID = 0, 1, 2, 3   # omg_channel_op act
+
+
+class ScrfdDesc(C.Structure):
+    _fields_ = [("scores", C.c_void_p * OMG_SCRFD_MAX_LEVELS), ("boxes", C.c_void_p * OMG_SCRFD_MAX_LEVELS),
+                ("kps", C.c_void_p * OMG_SCRFD_MAX_LEVELS), ("stride", C.c_int32 * OMG_SCRFD_MAX_LEVELS),
+                ("fh", C.c_int32 * OMG_SCRFD_MAX_LEVELS), ("fw", C.c_int32 * OMG_SCRFD_MAX_LEVELS),
+                ("n_levels", C.c_int32), ("num_anchors", C.c_int32), ("det_thresh", C.c_float),
+                ("nms_thresh", C.c_float), ("det_scale", C.c_float), ("out", C.c_void_p), ("max_out", C.c_int32),
+                ("count", C.c_void_p)]
+
+
 class FuseDesc(C.Structure):
     _fields_ = [("noise_main", C.c_void_p), ("noise_concept", C.c_void_p * OMG_MAX_CONCEPTS),
                 ("mask", C.c_void_p * OMG_MAX_CONCEPTS), ("n_concepts", C.c_int32), ("guidance", C.c_float),
@@ -100,6 +114,12 @@ SYMBOLS = {
                                     C.c_longlong, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "omg_sam_postprocess": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "omg_channel_op": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                 C.c_void_p]),
+    "omg_pool2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                             C.c_int, C.c_int, C.c_void_p]),
+    "omg_scrfd_detect": (C.c_int, [C.POINTER(ScrfdDesc), C.c_void_p]),
     "omg_plan_create": (C.c_void_p, []),
     "omg_plan_destroy": (None, [C.c_void_p]),
     "omg_plan_record_begin": (C.c_int, [C.c_void_p]),

@@ -552,6 +552,88 @@ def ctx_mix(ctx, coef, out=None):
     return out
 
 
+def _rows(t):
+    """(B, H, W, C) view with unit channel stride and pixels in row-major order -> (B, H, W, row stride)."""
+    B, H, W, Cc = t.shape
+    assert t.stride(3) == 1 and t.stride(1) == t.stride(2) * W and t.stride(0) == t.stride(1) * H
+    return B, H, W, t.stride(2)
+
+
+def channel_op(x, scale=None, shift=None, act=L.CH_ACT_NONE, slope=None, addend=None, add_scale=1, act_after_add=False,
+               out=None):
+    """omg_channel_op over (B, H, W, C) fp16 views (rows may be strided along the channel axis): y = act(x * scale +
+    shift) + addend, or act(x * scale + shift + addend) with act_after_add.  The addend is read at nearest
+    (y // add_scale, x // add_scale).  x None reads as zero.  scale / shift / slope fp32 [C] or None."""
+    ref = x if x is not None else addend
+    _chk16(ref)
+    if x is not None:
+        B, H, W, ldx = _rows(x)
+    else:
+        B, Ha, Wa, _ = addend.shape
+        H, W, ldx = Ha * add_scale, Wa * add_scale, 0
+    Cc = ref.shape[3]
+    if out is None:
+        out = torch.empty((B, H, W, Cc), dtype=torch.float16, device=ref.device)
+    _, _, _, ldy = _rows(out)
+    ld_add = 0
+    if addend is not None:
+        _chk16(addend)
+        assert addend.shape == (B, H // add_scale, W // add_scale, Cc)
+        ld_add = _rows(addend)[3]
+    for v in (scale, shift, slope):
+        assert v is None or (v.is_cuda and v.dtype == torch.float32 and v.is_contiguous() and v.numel() >= Cc)
+    L.check(L.load().omg_channel_op(_ptr(x), ldx, out.data_ptr(), ldy, _ptr(scale), _ptr(shift), _ptr(slope),
+                                    _ptr(addend), ld_add, 0 if addend is None else add_scale, B, H, W, Cc, int(act),
+                                    int(act_after_add), _stream()), "omg_channel_op")
+    return out
+
+
+def pool2d_out_size(n, k, stride, pad, ceil_mode):
+    """Output extent of PyTorch / ONNX pooling along one axis."""
+    o = (n + 2 * pad - k + (stride - 1 if ceil_mode else 0)) // stride + 1
+    if ceil_mode and (o - 1) * stride >= n + pad:
+        o -= 1
+    return o
+
+
+def pool2d(x, k, stride, pad=0, ceil_mode=False, count_include_pad=True, is_max=True, out=None):
+    """omg_pool2d: max or average pooling of a contiguous (B, H, W, C) fp16 tensor, C % 8 == 0."""
+    _chk16(x)
+    assert x.is_contiguous()
+    B, H, W, Cc = x.shape
+    Ho, Wo = pool2d_out_size(H, k, stride, pad, ceil_mode), pool2d_out_size(W, k, stride, pad, ceil_mode)
+    if out is None:
+        out = torch.empty((B, Ho, Wo, Cc), dtype=torch.float16, device=x.device)
+    assert out.shape == (B, Ho, Wo, Cc) and out.is_contiguous()
+    L.check(L.load().omg_pool2d(x.data_ptr(), out.data_ptr(), B, H, W, Cc, k, stride, pad, int(ceil_mode),
+                                int(count_include_pad), int(is_max), _stream()), "omg_pool2d")
+    return out
+
+
+def scrfd_detect(levels, num_anchors, det_thresh, det_scale, nms_thresh=0.4):
+    """omg_scrfd_detect.  levels: list of (stride, fh, fw, scores, boxes, kps or None) with fp32 CUDA tensors of
+    fh * fw * num_anchors rows (1 / 4 / 10 values each).  Returns the fp32 [n, 15] rows (box, score, 5 key-points) in
+    NMS order (a device tensor: the count is read back once)."""
+    d = L.ScrfdDesc()
+    d.n_levels, d.num_anchors = len(levels), num_anchors
+    T = 0
+    for i, (s, fh, fw, sc, bx, kp) in enumerate(levels):
+        for t in (sc, bx, kp):
+            assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+        n = fh * fw * num_anchors
+        assert sc.numel() == n and bx.numel() == 4 * n and (kp is None or kp.numel() == 10 * n)
+        d.scores[i], d.boxes[i], d.kps[i] = sc.data_ptr(), bx.data_ptr(), _ptr(kp)
+        d.stride[i], d.fh[i], d.fw[i] = s, fh, fw
+        T += n
+    dev = levels[0][3].device
+    out = torch.empty((max(T, 1), 15), dtype=torch.float32, device=dev)
+    count = torch.zeros(1, dtype=torch.int32, device=dev)
+    d.det_thresh, d.nms_thresh, d.det_scale = float(det_thresh), float(nms_thresh), float(det_scale)
+    d.out, d.max_out, d.count = out.data_ptr(), out.shape[0], count.data_ptr()
+    L.check(L.load().omg_scrfd_detect(C.byref(d), _stream()), "omg_scrfd_detect")
+    return out[: int(count.item())]
+
+
 # ------------------------------------------------------------------ weight packing (host, once per model load)
 def pack_conv3x3_weight(w):
     """torch Conv2d weight [N, C, 3, 3] -> [N, 9*C] with K order (ky, kx, c)."""

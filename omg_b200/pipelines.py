@@ -702,10 +702,13 @@ class InstantidMultiConceptPipeline(_BasePipeline):
 
     def get_face_embedding(self, face_app, ref_image):
         """instantid_pipeline.py:757-767: the reference sorts detections by (x2-x0)*y2 - y1 ascending and takes the
-        first (documented quirk); kept as is."""
+        first (documented quirk); kept as is.  A photo without a face raises ValueError naming it (the reference fails
+        with an IndexError)."""
         import cv2
         import numpy as np
         from PIL import Image
         info = face_app.get(cv2.cvtColor(np.array(Image.open(ref_image).convert("RGB")), cv2.COLOR_RGB2BGR))
+        if len(info) == 0:
+            raise ValueError(f"no face detected in the reference photo {ref_image}")
         info = sorted(info, key=lambda x: (x["bbox"][2] - x["bbox"][0]) * x["bbox"][3] - x["bbox"][1])[0]
         return info["embedding"]
