@@ -168,8 +168,9 @@ int omg_attention(const omg_attn_desc* desc, void* stream);
 /*
  * GroupNorm(32 groups) over channels-last fp16, optional SiLU, input = channel-concatenation of (x1 | x2).
  * y[B, HW, C1+C2].  stats_ws: OMG_GN_WS_FLOATS(B) floats of scratch.  Deterministic: no atomics, results do not depend
- * on the batch position of an image.  Replaces torch GroupNorm + SiLU + torch.cat inside diffusers
- * ResnetBlock2D / Transformer2DModel / UNet up-blocks [3P] (call site src/pipelines/lora_pipeline.py:546-566).
+ * on the batch position of an image.  x1, x2, y and stats_ws 16 B aligned.  Replaces torch GroupNorm + SiLU + torch.cat
+ * inside diffusers ResnetBlock2D / Transformer2DModel / UNet up-blocks [3P] (call site
+ * src/pipelines/lora_pipeline.py:546-566).
  */
 #define OMG_GN_MAX_SPLITS 256
 #define OMG_GN_WS_FLOATS(B) ((B) * (2 * 2 * 2560 + 64 * OMG_GN_MAX_SPLITS))
@@ -181,17 +182,19 @@ int omg_groupnorm_bf16(const void* x1, int C1, const void* x2, int C2, int B, in
 
 /* Per-channel (sum, sum of squares) partials of a stored channels-last tensor x [B, HW, C], one float2 per channel per
  * 32-row block: out [B][ceil(HW/32)][C] - the layout omg_gemm's col_stats_out produces (for tensors that were modified
- * after their producing GEMM, e.g. skip connections that received ControlNet residuals). */
+ * after their producing GEMM, e.g. skip connections that received ControlNet residuals).  x 4 B, out 16 B aligned. */
 int omg_colstats(const void* x, int C, int B, int HW, void* out, void* stream);
 
 /* GroupNorm(32) [+ SiLU] of cat(x1 | x2) from per-channel partials (omg_gemm col_stats_out / omg_colstats): one tiny
  * reduction launch (partials -> mean, rstd per image and group, fixed summation order) and one apply pass.
- * part1 [B][rb1][C1] float2, part2 [B][rb2][C2] float2 (NULL when C2 == 0); stats_ws: OMG_GN_WS_FLOATS(B) floats. */
+ * part1 [B][rb1][C1] float2, part2 [B][rb2][C2] float2 (NULL when C2 == 0), 8 B aligned; stats_ws: OMG_GN_WS_FLOATS(B)
+ * floats.  x1, x2, y and stats_ws 16 B aligned. */
 int omg_groupnorm_apply(const void* x1, int C1, const void* part1, int rb1, const void* x2, int C2, const void* part2,
                         int rb2, int B, int HW, const void* gamma, const void* beta, float eps, int silu, void* stats_ws,
                         void* y, void* stream);
 
-/* LayerNorm over the last dim of [rows, C] fp16 (BasicTransformerBlock norm1/2/3 [3P]). */
+/* LayerNorm over the last dim of [rows, C] fp16 (BasicTransformerBlock norm1/2/3 [3P]).  x, gamma, beta and y 16 B
+ * aligned. */
 int omg_layernorm(const void* x, const void* gamma, const void* beta, void* y, long long rows, int C, float eps,
                   void* stream);
 
@@ -207,6 +210,7 @@ int omg_layernorm(const void* x, const void* gamma, const void* beta, void* y, l
  *   eps = eps_u + guidance * (eps_c - eps_u);  latents += eps * (sigma_next - sigma)   (fp32 state [2, HW, 4]);
  *   next_main_in [4, HW, 8] = latents / sqrt(sigma_next^2 + 1) in row order (img0, img1, img0, img1);
  *   next_concept_in [2, HW, 8] = scaled image-1 latent twice; latents_f16 optional fp16 copy [2, HW, 4].
+ * Alignment: noise_main and noise_concept 8 B; latents, next_main_in and next_concept_in 16 B; latents_f16 4 B.
  */
 typedef struct {
     const void* noise_main;
@@ -231,14 +235,15 @@ int omg_fuse_step(const omg_fuse_desc* desc, void* stream);
  */
 int omg_ctx_mix(const void* ctx, const void* coef, void* out, int B, int L, int C, void* stream);
 
-/* y = a + alpha * b over n fp16 elements (n % 8 == 0): ControlNet residual injection
+/* y = a + alpha * b over n fp16 elements (n % 8 == 0; a, b, y 16 B aligned): ControlNet residual injection
  * (down_block_additional_residuals / mid_block_additional_residual, src/pipelines/lora_pipeline.py:546-556). */
 int omg_axpy(const void* a, const void* b, float alpha, void* y, long long n, void* stream);
 
 /* In-place row softmax: x[r, :cols] = softmax(scale * x[r, :cols]) for an fp16 matrix with row stride ld (elements),
- * fp32 arithmetic; cols % 8 == 0, cols <= 32768, scale > 0.  The VAE decoder's mid-block attention (one head of
- * 512 channels: `Attention(heads=1)` inside diffusers' AutoencoderKL, reached from src/pipelines/lora_pipeline.py:649)
- * materialises its scores with omg_gemm, normalises them here and applies them with a second omg_gemm. */
+ * fp32 arithmetic; cols % 8 == 0, cols <= 32768, scale > 0, x 16 B aligned.  The VAE decoder's mid-block attention
+ * (one head of 512 channels: `Attention(heads=1)` inside diffusers' AutoencoderKL, reached from
+ * src/pipelines/lora_pipeline.py:649) materialises its scores with omg_gemm, normalises them here and applies them with
+ * a second omg_gemm. */
 int omg_softmax_rows(void* x, long long rows, int cols, long long ld, float scale, void* stream);
 /* omg_softmax_rows over a bf16 matrix: same arguments and limits, fp32 arithmetic. */
 int omg_softmax_rows_bf16(void* x, long long rows, int cols, long long ld, float scale, void* stream);
@@ -254,6 +259,8 @@ int omg_softmax_rows_bf16(void* x, long long rows, int cols, long long ld, float
  *   omg_relu_linear_attention: LiteMLA.relu_linear_att (ops.py:404-440): per head (q | k | v, dim 32)
  *     out = relu(q) (relu(k)^T [v | 1]) normalised by its last column + eps; qkv [B, N, heads*96] -> out [B, N, heads*32].
  *   omg_resize_bicubic: F.interpolate(mode="bicubic", align_corners=False) (SamNeck inputs, sam.py:117-123).
+ * The fp16 tensors these read and write 8 channels at a time - x, w, bias and y of omg_dwconv, x and y of omg_group1x1 and
+ * omg_resize_bicubic - must be 16 B aligned.
  */
 int omg_dwconv(const void* x, const void* w, const void* bias, void* y, int B, int H, int W, int C, int ldx, int ldy, int ksize,
                int stride, int act, void* stream);
@@ -336,7 +343,8 @@ int omg_attention_relpos(const omg_attn_relpos_desc* desc, void* stream);
  *   NULL (read as 0: a nearest up-sampling on its own), scale / shift NULL (1 / 0).  act: OMG_CH_ACT_*; PReLU reads
  *   slope[c].  scale, shift and slope are fp32 [C].  y may alias x; it must not overlap the addend.
  * omg_pool2d: max (is_max = 1) or average pooling, k x k window (1 <= k <= 3), stride 1 | 2, symmetric pad < k, with
- *   ONNX / PyTorch ceil_mode and count_include_pad.  x [B, H, W, C] and y [B, Ho, Wo, C] contiguous, C % 8 == 0.
+ *   ONNX / PyTorch ceil_mode and count_include_pad.  x [B, H, W, C] and y [B, Ho, Wo, C] contiguous and 16 B aligned,
+ *   C % 8 == 0.
  * omg_scrfd_detect: SCRFD.detect after the network, in one CTA: anchors with score >= det_thresh (strides' row-major
  *   grids, num_anchors consecutive anchors per cell, centre (x, y) * stride), distance2bbox / distance2kps of the
  *   predictions times the stride, / det_scale, a descending sort of the scores (ties: lower anchor index first) and

@@ -242,6 +242,7 @@ static int softmax_rows_impl(void* x, long long rows, int cols, long long ld, fl
               "%s: cols=%d must be a multiple of 8 and <= %d, ld a multiple of 8", who, cols,
               SM_THREADS * SM_MAXV * 8);
     OMG_CHECK(scale > 0.f, "%s: scale must be positive", who);
+    if (check_aligned(who, 16, {{"x", x}})) return 1;
     OMG_CUDA(launch_pdl(softmax_rows_kernel<T>, dim3((unsigned)rows), dim3(SM_THREADS), 0, stream,
                         static_cast<T*>(x), cols, ld, scale * 1.4426950408889634f));
     return check_launch("softmax_rows_kernel");
@@ -250,6 +251,7 @@ static int softmax_rows_impl(void* x, long long rows, int cols, long long ld, fl
 static int axpy_impl(const void* a, const void* b, float alpha, void* y, long long n, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(a && b && y && n > 0 && n % 8 == 0, "omg_axpy: bad arguments");
+    if (check_aligned("omg_axpy", 16, {{"a", a}, {"b", b}, {"y", y}})) return 1;
     const long long nvec = n / 8;
     OMG_CUDA(launch_pdl(axpy_kernel, dim3((unsigned)((nvec + 255) / 256)), dim3(256), 0, stream,
                         static_cast<const uint4*>(a), static_cast<const uint4*>(b), alpha, static_cast<uint4*>(y), nvec));
@@ -262,6 +264,11 @@ static int fuse_step_impl(const omg_fuse_desc* d, void* stream_) {
     OMG_CHECK(d->n_concepts >= 0 && d->n_concepts <= OMG_MAX_CONCEPTS, "omg_fuse_step: n_concepts=%d out of range",
               d->n_concepts);
     OMG_CHECK(d->HW >= 1, "omg_fuse_step: empty latent");
+    if (check_aligned("omg_fuse_step", 16, {{"latents", d->latents}, {"next_main_in", d->next_main_in},
+                                            {"next_concept_in", d->next_concept_in}}) ||
+        check_aligned("omg_fuse_step", 8, {{"noise_main", d->noise_main}}) ||
+        check_aligned("omg_fuse_step", 4, {{"latents_f16", d->latents_f16}}))
+        return 1;
     FuseParams p;
     p.noise_main = static_cast<const __half*>(d->noise_main);
     for (int k = 0; k < OMG_MAX_CONCEPTS; ++k) {
@@ -269,6 +276,7 @@ static int fuse_step_impl(const omg_fuse_desc* d, void* stream_) {
         p.mask[k] = k < d->n_concepts ? static_cast<const float*>(d->mask[k]) : nullptr;
         OMG_CHECK(k >= d->n_concepts || p.mask[k] == nullptr || p.noise_concept[k] != nullptr,
                   "omg_fuse_step: concept %d has a mask but no noise prediction", k);
+        if (check_aligned("omg_fuse_step", 8, {{"noise_concept", p.noise_concept[k]}})) return 1;
     }
     p.n_concepts = d->n_concepts;
     p.guidance = d->guidance;

@@ -281,6 +281,7 @@ static int pool2d_impl(const void* x, void* y, int B, int H, int W, int C, int k
                        int count_include_pad, int is_max, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && y, "omg_pool2d: null pointer");
+    if (check_aligned("omg_pool2d", 16, {{"x", x}, {"y", y}})) return 1;
     OMG_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 8 && C % 8 == 0, "omg_pool2d: bad shape (C=%d must be a multiple of 8)", C);
     OMG_CHECK(k >= 1 && k <= 3 && (stride == 1 || stride == 2) && pad >= 0 && 2 * pad <= k,
               "omg_pool2d: kernel %d, stride %d, pad %d unsupported (k <= 3, stride 1 | 2, pad <= k / 2)", k, stride, pad);

@@ -8,6 +8,8 @@
 
 #include <atomic>
 #include <functional>
+#include <initializer_list>
+#include <utility>
 
 namespace omg {
 
@@ -36,6 +38,16 @@ inline int check_head_windows(const char* who, int heads, int head_dim, const in
         if (col0[i] < 0 || col0[i] + width > ld[i])
             return fail("%s: %s head window [%d, %lld) does not fit its row of %d elements", who, names[i], col0[i],
                         col0[i] + width, ld[i]);
+    return 0;
+}
+
+// Kernels that move 4 / 8 / 16 B vectors through a caller's pointer need it aligned to that width: a misaligned vector
+// access is a sticky fault that takes down the CUDA context of the whole process, so the entry point rejects it first.
+// NULL (an absent optional operand) passes.
+inline int check_aligned(const char* who, int bytes, std::initializer_list<std::pair<const char*, const void*>> ptrs) {
+    for (const auto& p : ptrs)
+        if (reinterpret_cast<uintptr_t>(p.second) % (uintptr_t)bytes != 0)
+            return fail("%s: %s must be %d B aligned", who, p.first, bytes);
     return 0;
 }
 

@@ -392,6 +392,7 @@ static int groupnorm_impl(const void* x1, int C1, const void* x2, int C2, int B,
     const int C = C1 + C2;
     const char* who = std::is_same_v<T, __half> ? "omg_groupnorm" : "omg_groupnorm_bf16";
     OMG_CHECK(x1 && gamma && beta && stats_ws && y, "%s: null pointer", who);
+    if (check_aligned(who, 16, {{"x1", x1}, {"x2", x2}, {"y", y}, {"stats_ws", stats_ws}})) return 1;
     OMG_CHECK(C1 > 0 && C1 % 8 == 0 && C2 >= 0 && C2 % 8 == 0 && (C2 == 0 || x2), "%s: bad channel split", who);
     OMG_CHECK(C % 32 == 0 && C <= 2560, "%s: C=%d must be a multiple of 32 and <= 2560", who, C);
     OMG_CHECK(B >= 1 && HW >= 1, "%s: empty input", who);
@@ -431,6 +432,7 @@ static int groupnorm_impl(const void* x1, int C1, const void* x2, int C2, int B,
 static int colstats_impl(const void* x, int C, int B, int HW, void* out, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && out, "omg_colstats: null pointer");
+    if (check_aligned("omg_colstats", 4, {{"x", x}}) || check_aligned("omg_colstats", 16, {{"out", out}})) return 1;
     OMG_CHECK(C >= 8 && C % 8 == 0 && B >= 1 && HW >= 1, "omg_colstats: bad shape");
     const int rbs = (HW + 31) / 32;
     OMG_CUDA(launch_pdl(colstats_kernel, dim3((rbs + 7) / 8, B), dim3(256), 0, stream, static_cast<const __half*>(x), C, HW,
@@ -444,6 +446,9 @@ static int groupnorm_apply_impl(const void* x1, int C1, const void* part1, int r
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const int C = C1 + C2;
     OMG_CHECK(x1 && part1 && gamma && beta && stats_ws && y, "omg_groupnorm_apply: null pointer");
+    if (check_aligned("omg_groupnorm_apply", 16, {{"x1", x1}, {"x2", x2}, {"y", y}, {"stats_ws", stats_ws}}) ||
+        check_aligned("omg_groupnorm_apply", 8, {{"part1", part1}, {"part2", part2}}))
+        return 1;
     OMG_CHECK(C1 > 0 && C1 % 8 == 0 && C2 >= 0 && C2 % 8 == 0 && (C2 == 0 || (x2 && part2)), "omg_groupnorm_apply: bad channel split");
     OMG_CHECK(C % 32 == 0 && C <= 2560, "omg_groupnorm_apply: C=%d must be a multiple of 32 and <= 2560", C);
     OMG_CHECK(B >= 1 && HW >= 1 && rb1 >= 1 && (C2 == 0 || rb2 >= 1), "omg_groupnorm_apply: empty input");
@@ -461,6 +466,7 @@ static int layernorm_impl(const void* x, const void* gamma, const void* beta, vo
                              float eps, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && gamma && beta && y, "omg_layernorm: null pointer");
+    if (check_aligned("omg_layernorm", 16, {{"x", x}, {"y", y}, {"gamma", gamma}, {"beta", beta}})) return 1;
     OMG_CHECK(C % 8 == 0 && C >= 8 && C <= 2560, "omg_layernorm: C=%d unsupported", C);
     OMG_CHECK(rows >= 1, "omg_layernorm: empty input");
     const int warps = 8;

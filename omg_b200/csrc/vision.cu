@@ -244,6 +244,7 @@ static int dwconv_impl(const void* x, const void* w, const void* bias, void* y, 
                           int ksize, int stride, int act, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && w && y, "omg_dwconv: null pointer");
+    if (check_aligned("omg_dwconv", 16, {{"x", x}, {"w", w}, {"bias", bias}, {"y", y}})) return 1;
     OMG_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 8 && C % 8 == 0, "omg_dwconv: bad shape (C must be a multiple of 8)");
     OMG_CHECK(ldx >= C && ldy >= C && ldx % 8 == 0 && ldy % 8 == 0, "omg_dwconv: row strides must be >= C and multiples of 8");
     OMG_CHECK((ksize == 3 || ksize == 5) && (stride == 1 || stride == 2) && (act == 0 || act == 1), "omg_dwconv: kernel 3|5, stride 1|2, act 0|1");
@@ -263,6 +264,7 @@ static int group1x1_impl(const void* x, const void* w, void* y, long long pixels
                             void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && w && y, "omg_group1x1: null pointer");
+    if (check_aligned("omg_group1x1", 16, {{"x", x}, {"y", y}})) return 1;
     OMG_CHECK(group == 32 && C >= 32 && C % 32 == 0 && pixels >= 1, "omg_group1x1: group size 32, C a multiple of 32");
     OMG_CHECK(ldx >= C && ldy >= C && ldx % 8 == 0 && ldy % 8 == 0, "omg_group1x1: row strides must be >= C and multiples of 8");
     const dim3 grid((unsigned)((pixels + 63) / 64), C / 32);
@@ -283,6 +285,7 @@ static int relu_linear_attention_impl(const void* qkv, void* out, int B, int N, 
 static int resize_bicubic_impl(const void* x, void* y, int B, int H, int W, int C, int Ho, int Wo, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     OMG_CHECK(x && y, "omg_resize_bicubic: null pointer");
+    if (check_aligned("omg_resize_bicubic", 16, {{"x", x}, {"y", y}})) return 1;
     OMG_CHECK(B >= 1 && H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1 && C >= 8 && C % 8 == 0, "omg_resize_bicubic: bad shape");
     const long long total = (long long)Ho * Wo * (C / 8);
     OMG_CUDA(launch_pdl(resize_bicubic_kernel, dim3((unsigned)((total + 255) / 256), B), dim3(256), 0, stream,

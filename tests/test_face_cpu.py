@@ -227,6 +227,27 @@ def test_face_c_abi_rejects_bad_arguments_before_touching_the_gpu():
     assert "null descriptor" in err(lib.omg_scrfd_detect(None, None))
 
 
+def test_pool2d_out_size_equals_torch_output_shape():
+    """ops.pool2d_out_size (the host's copy of omg_pool2d's output extent) against torch's max / avg pooling, for every
+    window the entry point accepts and inputs of 1 to 12 pixels."""
+    from omg_b200 import ops
+    n_checked = 0
+    for n in range(1, 13):
+        for k in (1, 2, 3):
+            for stride in (1, 2):
+                for pad in (0, 1):
+                    if 2 * pad > k or n + 2 * pad < k:
+                        continue
+                    for ceil in (False, True):
+                        x = torch.zeros(1, 1, n, n + 1)
+                        want = torch.nn.functional.max_pool2d(x, k, stride, pad, ceil_mode=ceil).shape[2:]
+                        assert want == torch.nn.functional.avg_pool2d(x, k, stride, pad, ceil_mode=ceil).shape[2:]
+                        got = (ops.pool2d_out_size(n, k, stride, pad, ceil), ops.pool2d_out_size(n + 1, k, stride, pad, ceil))
+                        assert got == tuple(want), (n, k, stride, pad, ceil)
+                        n_checked += 1
+    assert n_checked == 228
+
+
 def test_face_cu_compiles_without_spills():
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     from omg_b200 import build as b

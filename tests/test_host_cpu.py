@@ -288,6 +288,77 @@ def test_c_abi_rejects_bad_arguments_before_touching_the_gpu():
     assert "bad channel split" in err(lib.omg_groupnorm(fake, 100, None, 0, 1, 16, fake, fake, 1e-5, 0, fake, fake, None))
 
 
+def test_c_abi_rejects_misaligned_vector_operands_before_touching_the_gpu():
+    """Entry points whose kernels move 4 / 8 / 16 B vectors through a pointer reject one that is not aligned to that width
+    with an error status (a misaligned vector access would be a sticky fault of the whole CUDA context).  Every other
+    argument is valid, so without the check each call would go on to launch; none does."""
+    import ctypes as C
+    from omg_b200 import _lib as L
+    lib = L.load()
+    ok, off8, off4, off2 = 0x1000, 0x1008, 0x1004, 0x1002
+
+    def fuse(**ptrs):
+        f = L.FuseDesc()
+        f.n_concepts, f.HW, f.sigma, f.sigma_next, f.guidance = 1, 64, 1.0, 0.5, 7.5
+        f.noise_main = f.latents = f.next_main_in = f.next_concept_in = f.latents_f16 = ok
+        f.noise_concept[0] = f.mask[0] = ok
+        for k, v in ptrs.items():
+            if k == "noise_concept":
+                f.noise_concept[0] = v
+            else:
+                setattr(f, k, v)
+        return lib.omg_fuse_step(C.byref(f), None)
+
+    gn = lambda name, x1, x2, y, ws: getattr(lib, name)(x1, 64, x2, 32, 1, 16, ok, ok, 1e-5, 0, ws, y, None)  # noqa: E731
+    gna = lambda x1, p1, p2, y: lib.omg_groupnorm_apply(x1, 64, p1, 1, ok, 32, p2, 1, 1, 16, ok, ok, 1e-5, 0, ok, y,  # noqa: E731
+                                                        None)
+    cases = [
+        (lambda: lib.omg_pool2d(off8, ok, 1, 4, 4, 8, 3, 2, 1, 0, 1, 1, None), "omg_pool2d: x must be 16 B aligned"),
+        (lambda: lib.omg_pool2d(ok, off2, 1, 4, 4, 8, 3, 2, 1, 0, 1, 0, None), "omg_pool2d: y must be 16 B aligned"),
+        (lambda: lib.omg_dwconv(off8, ok, ok, ok, 1, 4, 4, 8, 8, 8, 3, 1, 0, None), "omg_dwconv: x must be 16 B"),
+        (lambda: lib.omg_dwconv(ok, off8, ok, ok, 1, 4, 4, 8, 8, 8, 3, 1, 0, None), "omg_dwconv: w must be 16 B"),
+        (lambda: lib.omg_dwconv(ok, ok, off2, ok, 1, 4, 4, 8, 8, 8, 5, 2, 1, None), "omg_dwconv: bias must be 16 B"),
+        (lambda: lib.omg_dwconv(ok, ok, None, off8, 1, 4, 4, 8, 8, 8, 3, 1, 0, None), "omg_dwconv: y must be 16 B"),
+        (lambda: lib.omg_group1x1(off8, ok, ok, 16, 32, 32, 32, 32, None), "omg_group1x1: x must be 16 B"),
+        (lambda: lib.omg_group1x1(ok, ok, off8, 16, 32, 32, 32, 32, None), "omg_group1x1: y must be 16 B"),
+        (lambda: lib.omg_resize_bicubic(off8, ok, 1, 4, 4, 8, 8, 8, None), "omg_resize_bicubic: x must be 16 B"),
+        (lambda: lib.omg_resize_bicubic(ok, off2, 1, 4, 4, 8, 8, 8, None), "omg_resize_bicubic: y must be 16 B"),
+        (lambda: gn("omg_groupnorm", off8, ok, ok, ok), "omg_groupnorm: x1 must be 16 B"),
+        (lambda: gn("omg_groupnorm", ok, off8, ok, ok), "omg_groupnorm: x2 must be 16 B"),
+        (lambda: gn("omg_groupnorm", ok, ok, off2, ok), "omg_groupnorm: y must be 16 B"),
+        (lambda: gn("omg_groupnorm", ok, ok, ok, off8), "omg_groupnorm: stats_ws must be 16 B"),
+        (lambda: gn("omg_groupnorm_bf16", off8, ok, ok, ok), "omg_groupnorm_bf16: x1 must be 16 B"),
+        (lambda: gn("omg_groupnorm_bf16", ok, ok, off8, ok), "omg_groupnorm_bf16: y must be 16 B"),
+        (lambda: gna(off8, ok, ok, ok), "omg_groupnorm_apply: x1 must be 16 B"),
+        (lambda: gna(ok, ok, ok, off8), "omg_groupnorm_apply: y must be 16 B"),
+        (lambda: gna(ok, off4, ok, ok), "omg_groupnorm_apply: part1 must be 8 B"),
+        (lambda: gna(ok, ok, off4, ok), "omg_groupnorm_apply: part2 must be 8 B"),
+        (lambda: lib.omg_colstats(off2, 64, 1, 16, ok, None), "omg_colstats: x must be 4 B"),
+        (lambda: lib.omg_colstats(ok, 64, 1, 16, off8, None), "omg_colstats: out must be 16 B"),
+        (lambda: lib.omg_layernorm(off8, ok, ok, ok, 4, 64, 1e-5, None), "omg_layernorm: x must be 16 B"),
+        (lambda: lib.omg_layernorm(ok, off8, ok, ok, 4, 64, 1e-5, None), "omg_layernorm: gamma must be 16 B"),
+        (lambda: lib.omg_layernorm(ok, ok, off2, ok, 4, 64, 1e-5, None), "omg_layernorm: beta must be 16 B"),
+        (lambda: lib.omg_layernorm(ok, ok, ok, off8, 4, 64, 1e-5, None), "omg_layernorm: y must be 16 B"),
+        (lambda: lib.omg_softmax_rows(off8, 4, 64, 64, 1.0, None), "omg_softmax_rows: x must be 16 B"),
+        (lambda: lib.omg_softmax_rows_bf16(off2, 4, 64, 64, 1.0, None), "omg_softmax_rows_bf16: x must be 16 B"),
+        (lambda: lib.omg_axpy(off8, ok, 0.5, ok, 64, None), "omg_axpy: a must be 16 B"),
+        (lambda: lib.omg_axpy(ok, off8, 0.5, ok, 64, None), "omg_axpy: b must be 16 B"),
+        (lambda: lib.omg_axpy(ok, ok, 0.5, off2, 64, None), "omg_axpy: y must be 16 B"),
+        (lambda: fuse(latents=off8), "omg_fuse_step: latents must be 16 B"),
+        (lambda: fuse(next_main_in=off8), "omg_fuse_step: next_main_in must be 16 B"),
+        (lambda: fuse(next_concept_in=off8), "omg_fuse_step: next_concept_in must be 16 B"),
+        (lambda: fuse(noise_main=off4), "omg_fuse_step: noise_main must be 8 B"),
+        (lambda: fuse(noise_concept=off4), "omg_fuse_step: noise_concept must be 8 B"),
+        (lambda: fuse(latents_f16=off2), "omg_fuse_step: latents_f16 must be 4 B"),
+    ]
+    for call, msg in cases:
+        n0 = lib.omg_launch_count()
+        rc = call()
+        e = lib.omg_last_error().decode()
+        assert rc == 1 and e.startswith(msg), (msg, rc, e)
+        assert lib.omg_launch_count() == n0, msg
+
+
 def test_cli_flags_match_the_reference_parse_args():
     """Every flag of the reference CLIs (inference_lora.py:203-222, inference_instantid.py:259-286; names, defaults and
     types extracted from the reference files by tests/golden/make_golden.py) exists here with the same default;
