@@ -299,6 +299,8 @@ class OnnxNet:
             for kx in range(kw):
                 ry, rx = ky - ph, kx - pw
                 phase, dy, dx = ((0, 0), ry, rx) if s == 1 else ((ry % 2, rx % 2), ry // 2, rx // 2)
+                if phase[0] >= H or phase[1] >= W:
+                    continue   # an input side of 1 pixel leaves the odd phase empty: such a tap reads only padding
                 if phase not in vidx:
                     vidx[phase] = len(views)
                     views.append(ops.view4(x.t if s == 1 else x.t[:, phase[0]::2, phase[1]::2, :]))

@@ -230,9 +230,10 @@ def conv3x3(x, w, bias=None, rowvec=None, residual=None, out=None, shortcut=None
     return out
 
 
-def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None, row_groups=None):
+def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None, row_groups=None, epilogue=L.EPI_NONE):
     """3x3 / stride 2 / pad 1 conv (Downsample2D): A operands are the four stride-2 phase views of x.
-    row_groups: per-stream weight planes, see conv3x3."""
+    row_groups: per-stream weight planes, see conv3x3.  epilogue: activation applied after the bias (the tanh-GELU of the
+    SAM encoder's stride-2 convs)."""
     B, H, W, Cin = x.shape
     N, Ktot = w.shape
     if row_groups is not None:
@@ -247,7 +248,7 @@ def conv3x3_s2(x, w, bias=None, out=None, block_n=0, colstats=None, row_groups=N
             py, oy = (1, -1) if ky == 0 else ((0, 0) if ky == 1 else (1, 0))
             px, ox = (1, -1) if kx == 0 else ((0, 0) if kx == 1 else (1, 0))
             segs.append((py * 2 + px, ox, oy, 0, Cin, (ky * 3 + kx) * Cin))
-    gemm(views, segs, w, N, Ktot, view4(out), bias=bias, block_n=block_n,
+    gemm(views, segs, w, N, Ktot, view4(out), bias=bias, epilogue=epilogue, block_n=block_n,
          colstats=None if colstats is None else (colstats, 0), row_groups=_image_groups(row_groups, (H // 2) * (W // 2)))
     return out
 

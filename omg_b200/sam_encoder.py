@@ -74,28 +74,11 @@ class _Conv:
             return y
         if self.stride == 2:
             assert residual is None and not (H % 2 or W % 2)
-            y = ops.conv3x3_s2(x, self.w, bias=self.bias, out=out) if not self.act else _conv_s2_act(x, self.w, self.bias, epi)
-            return y
+            return ops.conv3x3_s2(x, self.w, bias=self.bias, out=out, epilogue=epi)
         y = out if out is not None else torch.empty((B, H, W, self.n), dtype=torch.float16, device=x.device)
         ops.gemm([ops.view4(x)], ops._taps3x3(x.shape[3]), self.w, self.n, self.w.shape[1], ops.view4(y), bias=self.bias,
                  residual=residual, residual_ld=0 if residual is None else self.n, epilogue=epi)
         return y
-
-
-def _conv_s2_act(x, w, bias, epi):
-    """3x3 / stride 2 conv with an activation epilogue (ops.conv3x3_s2 has none): same phase-view segments."""
-    B, H, W, Cin = x.shape
-    N, Ktot = w.shape
-    out = torch.empty((B, H // 2, W // 2, N), dtype=torch.float16, device=x.device)
-    views = [ops.view4(x[:, py::2, px::2, :]) for py in range(2) for px in range(2)]
-    segs = []
-    for ky in range(3):
-        for kx in range(3):
-            py, oy = (1, -1) if ky == 0 else ((0, 0) if ky == 1 else (1, 0))
-            px, ox = (1, -1) if kx == 0 else ((0, 0) if kx == 1 else (1, 0))
-            segs.append((py * 2 + px, ox, oy, 0, Cin, (ky * 3 + kx) * Cin))
-    ops.gemm(views, segs, w, N, Ktot, ops.view4(out), bias=bias, epilogue=epi)
-    return out
 
 
 class _LiteMLA:

@@ -231,12 +231,15 @@ class PackedUNet:
             return torch.cat(As, dim=0), torch.cat(Bs, dim=1)
 
         def put(key_out, parts, geglu=False):
-            """parts: list of (A_cat [R_i,in], B [N_i,R_i]) for row blocks of a fused weight."""
+            """parts: list of (A_cat [R_i,in], B [N_i,R_i]) for row blocks of a fused weight.  The summed rank is padded
+            to a multiple of 8 with zero rows of A and zero columns of B2 (exact): t = A x is a GEMM output with r_tot
+            channels and B2 a weight matrix with r_tot columns, and omg_gemm takes both only in multiples of 8."""
             if all(p is None for p in parts["ab"]):
                 return
             As, rows = [], []
             r_off = 0
-            r_tot = sum(0 if ab is None else ab[0].shape[0] for ab in parts["ab"])
+            r_sum = sum(0 if ab is None else ab[0].shape[0] for ab in parts["ab"])
+            r_tot = (r_sum + 7) // 8 * 8
             dev0 = next(ab[0].device for ab in parts["ab"] if ab is not None)
             for ab, n_rows in zip(parts["ab"], parts["rows"]):
                 blk = torch.zeros(n_rows, r_tot, device=dev0)
@@ -246,6 +249,8 @@ class PackedUNet:
                     blk[:, r_off:r_off + A.shape[0]] = Bm
                     r_off += A.shape[0]
                 rows.append(blk)
+            if r_tot > r_sum:
+                As.append(As[0].new_zeros(r_tot - r_sum, As[0].shape[1]))
             B2 = torch.cat(rows, dim=0)
             if geglu:
                 B2, _ = ops.pack_geglu_weight(B2)
