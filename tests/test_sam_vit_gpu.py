@@ -35,8 +35,9 @@ def _nan_rows(t, extra=8):
     return buf[extra // 2:extra // 2 + t.shape[0]]
 
 
-def relpos_reference(qkv, H, W, heads, hd, th, tw, window, bias):
-    """float64 (B, H*W, C): segment_anything Attention after qkv, with window_partition's padding made of qkv(0) = bias."""
+def relpos_reference(qkv, H, W, heads, hd, th, tw, window, bias, scale=None):
+    """float64 (B, H*W, C): segment_anything Attention after qkv, with window_partition's padding made of qkv(0) = bias
+    (scale None: head_dim^-0.5)."""
     from oracle.sam_vit import attention_core, window_unpartition
     B, C = qkv.shape[0], heads * hd
     x = qkv.double().view(B, H, W, 3 * C)
@@ -45,10 +46,10 @@ def relpos_reference(qkv, H, W, heads, hd, th, tw, window, bias):
         full = bias.double().view(1, 1, 1, 3 * C).expand(B, Hp, Wp, 3 * C).clone()
         full[:, :H, :W] = x
         wins = full.view(B, Hp // window, window, Wp // window, window, 3 * C).permute(0, 1, 3, 2, 4, 5)
-        y = attention_core(wins.reshape(-1, window, window, 3 * C), heads, th.double(), tw.double())
+        y = attention_core(wins.reshape(-1, window, window, 3 * C), heads, th.double(), tw.double(), scale)
         y = window_unpartition(y, window, (Hp, Wp), (H, W))
     else:
-        y = attention_core(x, heads, th.double(), tw.double())
+        y = attention_core(x, heads, th.double(), tw.double(), scale)
     return y.reshape(B, H * W, C)
 
 
