@@ -228,6 +228,29 @@ typedef struct {
 int omg_fuse_step(const omg_fuse_desc* desc, void* stream);
 
 /*
+ * omg_fuse_step with a general one-step sampler update in place of Euler's, in a single launch: the scheduler step
+ * of diffusers' EulerDiscreteScheduler (any prediction type), EulerAncestralDiscreteScheduler and
+ * DPMSolverMultistepScheduler (dpmsolver++ / sde-dpmsolver++, orders 1 and 2) in coefficient form [3P]
+ * (lora_pipeline.py:615 `self.scheduler.step`).  Per element of each image, with eps the fused, guided prediction:
+ *   x0 = c_x * x + c_eps * eps;   x' = a * x + b * x0 + c * h + d * z;   latents = x';
+ *   next inputs = x' * input_scale (same rows as omg_fuse_step); latents_f16 as omg_fuse_step.
+ *   h = history [2, HW, 4] fp32, read when c != 0, then overwritten with x0 when store_x0 != 0;
+ *   z = noise, fp16 in NCHW [2, 4, HW] (the layout torch.randn((2, 4, h, w)) draws), read when d != 0.
+ * fuse.sigma / fuse.sigma_next are unused.  Alignment: as omg_fuse_step; history 16 B, noise 2 B.
+ */
+typedef struct {
+    omg_fuse_desc fuse;
+    float c_x, c_eps;
+    float a, b, c, d;
+    float input_scale;
+    void* history;
+    const void* noise;
+    int32_t store_x0;
+} omg_solver_desc;
+
+int omg_solver_step(const omg_solver_desc* desc, void* stream);
+
+/*
  * out[b, w, :] = sum_n coef[w, n] * ctx[b, n, :]  (fp16 ctx/out [B, L, C], fp32 coef [L, L]).  Builds the
  * prompt-to-prompt edited context  M diag(alpha) ctx  /  diag(1-alpha) ctx  so that the cross-attention edit
  * P0 M * alpha + (1-alpha) P1  (src/prompt_attention/p2p_attention.py:131-134,146-147) becomes two plain attention

@@ -28,6 +28,8 @@ import os
 import numpy as np
 import torch
 
+from omg_b200.scheduler import CLI_CHOICES as CLI_SCHEDULERS, cli_scheduler
+
 
 def draw_kps_multi(image_size, kps_list, color_list=((255, 0, 0), (0, 255, 0), (0, 0, 255), (255, 255, 0),
                                                      (255, 0, 255))):
@@ -102,6 +104,8 @@ def parse_args():
                    "rows before the first fusion step, stage-2 steps 0..15")
     p.add_argument("--synthetic", action="store_true", help="random-init SDXL-shaped weights, synthetic identities")
     p.add_argument("--tiny", action="store_true", help="with --synthetic: toy widths (plumbing check)")
+    p.add_argument("--scheduler", default=None, choices=list(CLI_SCHEDULERS),
+                   help="sampler, configured from the checkpoint's scheduler_config.json (default: that config as is)")
     p.add_argument("--num_inference_steps", default=50, type=int)
     p.add_argument("--image_size", default=1024, type=int)
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
@@ -277,6 +281,8 @@ if __name__ == "__main__":
             masks.append(m)
         masks = masks or [None] * len(regions)
     pipe.dedup = args.dedup
+    if args.scheduler:
+        pipe.scheduler = cli_scheduler(args.scheduler, pipe.scheduler.config)
     if args.decode:
         from omg_b200.vae import PackedVaeDecoder, VaeConfig
         if args.synthetic:

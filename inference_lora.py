@@ -22,6 +22,8 @@ import os
 
 import torch
 
+from omg_b200.scheduler import CLI_CHOICES as CLI_SCHEDULERS, cli_scheduler
+
 
 def prepare_text(prompt, region_prompts):
     """'[prompt]-*-[negative]|[prompt]-*-[negative]' -> (prompt, [(region, region_negative), ...])
@@ -75,6 +77,8 @@ def parse_args():
     p.add_argument("--dedup", action="store_true", help="skip work that repeats identical work (same outputs): twin "
                    "rows before the first fusion step, stage-2 steps 0..15")
     p.add_argument("--synthetic", action="store_true", help="random-init SDXL-shaped weights, synthetic encoders/masks")
+    p.add_argument("--scheduler", default=None, choices=list(CLI_SCHEDULERS),
+                   help="sampler, configured from the checkpoint's scheduler_config.json (default: that config as is)")
     p.add_argument("--num_inference_steps", default=50, type=int)
     p.add_argument("--image_size", default=1024, type=int)
     p.add_argument("--tiny", action="store_true", help="with --synthetic: toy widths (plumbing check)")
@@ -122,6 +126,7 @@ def build_model_sd(args, prompts, device):
     from omg_b200.config import UNetConfig
     from omg_b200.pipelines import ConceptModels, LoraMultiConceptPipeline, revise_regionally_controlnet_forward
     from omg_b200.prompt_attention import AttentionReplace
+    from omg_b200.scheduler import load_scheduler
     from omg_b200.text import ClipPromptEncoder
     from omg_b200.unet import PackedUNet
     cfg = UNetConfig.sdxl()
@@ -145,6 +150,7 @@ def build_model_sd(args, prompts, device):
         from omg_b200.vae import PackedVaeDecoder
         vae = PackedVaeDecoder.from_pretrained(args.pretrained_sdxl_model, "vae", dtype=torch.bfloat16, device=device)
     pipe = LoraMultiConceptPipeline(unet, controlnet=controlnet, prompt_encoder=enc, vae_decoder=vae)
+    pipe.scheduler = load_scheduler(args.pretrained_sdxl_model)  # the checkpoint's scheduler_config.json
     controller = AttentionReplace(prompts, 50, cross_replace_steps={"default_": 1.}, self_replace_steps=0.4,
                                   tokenizer=enc.tokenizer, width=args.image_size // 32, height=args.image_size // 32)
     revise_regionally_controlnet_forward(pipe, controller)
@@ -185,6 +191,8 @@ if __name__ == "__main__":
     build = build_model_synthetic if args.synthetic else build_model_sd
     pipe, controller, pipe_concepts, pipe_list, synth_masks = build(args, prompts, device)
     pipe.dedup = args.dedup
+    if args.scheduler:
+        pipe.scheduler = cli_scheduler(args.scheduler, pipe.scheduler.config)
     if args.synthetic and args.decode:
         from omg_b200 import synthetic
         from omg_b200.vae import PackedVaeDecoder, VaeConfig

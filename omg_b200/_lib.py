@@ -82,6 +82,12 @@ class FuseDesc(C.Structure):
                 ("HW", C.c_int32)]
 
 
+class SolverDesc(C.Structure):
+    _fields_ = [("fuse", FuseDesc), ("c_x", C.c_float), ("c_eps", C.c_float), ("a", C.c_float), ("b", C.c_float),
+                ("c", C.c_float), ("d", C.c_float), ("input_scale", C.c_float), ("history", C.c_void_p),
+                ("noise", C.c_void_p), ("store_x0", C.c_int32)]
+
+
 # every symbol include/omg_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "omg_gemm": (C.c_int, [C.POINTER(GemmDesc), C.c_void_p]),
@@ -99,6 +105,7 @@ SYMBOLS = {
     "omg_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_float,
                                 C.c_void_p]),
     "omg_fuse_step": (C.c_int, [C.POINTER(FuseDesc), C.c_void_p]),
+    "omg_solver_step": (C.c_int, [C.POINTER(SolverDesc), C.c_void_p]),
     "omg_ctx_mix": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "omg_axpy": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_longlong, C.c_void_p]),
     "omg_softmax_rows": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_float, C.c_void_p]),

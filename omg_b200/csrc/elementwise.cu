@@ -5,6 +5,10 @@
 // forcing a host sync through nonzero(); src/pipelines/instantid_pipeline.py:618-690 is identical).
 // Algorithmic bytes per launch (HW latent pixels, n concepts): read (4 + 2n) * HW*8*2 B noise + n * HW*4 B masks
 // + HW*2*4*4 B latents; write HW*2*4*4 B latents + 6 * HW*8*2 B next inputs.
+// omg_solver_step: the same fusion and guidance, then x0 = c_x x + c_eps eps and x' = a x + b x0 + c h + d z (the
+// Euler, Euler-ancestral and DPM-Solver++ 2M / 2M SDE steps in coefficient form, omg_b200/scheduler.py), sharing
+// one device body with omg_fuse_step.  On top of omg_fuse_step's bytes it reads HW*2*4*4 B history (c != 0) and
+// HW*2*4*2 B noise (d != 0) and writes HW*2*4*4 B history (store_x0).
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -29,6 +33,17 @@ struct FuseParams {
     int HW;
 };
 
+// omg_solver_step: the same fusion and outputs, a general one-step update instead of Euler's
+struct SolverParams {
+    FuseParams f;                  // sigma / sigma_next unused
+    float c_x, c_eps;              // x0 = c_x x + c_eps eps
+    float a, b, c, d;              // x' = a x + b x0 + c h + d z
+    float in_scale;                // next inputs = x' * in_scale
+    float* history;                // [2, HW, 4] fp32: h in (when c != 0), x0 out (when store_x0)
+    const __half* noise;           // [2, 4, HW] fp16 NCHW z (when d != 0)
+    int store_x0;
+};
+
 __device__ __forceinline__ void load4(const __half* p, float (&v)[4]) {
     const uint2 u = *reinterpret_cast<const uint2*>(p);
     const __half2* h = reinterpret_cast<const __half2*>(&u);
@@ -36,11 +51,8 @@ __device__ __forceinline__ void load4(const __half* p, float (&v)[4]) {
     v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
 }
 
-__global__ void fuse_step_kernel(FuseParams p) {
-    griddep_launch_dependents();
-    griddep_wait();
-    const int pix = blockIdx.x * blockDim.x + threadIdx.x;
-    if (pix >= p.HW) return;
+// Region noise fusion + classifier-free guidance of one latent pixel: the guided predictions of images 0 and 1.
+__device__ __forceinline__ void fused_guided_eps(const FuseParams& p, int pix, float (&e0)[4], float (&e1)[4]) {
     const size_t HW = p.HW;
     float u0[4], u1[4], c0[4], c1[4];
     load4(p.noise_main + (0 * HW + pix) * 8, u0);
@@ -73,18 +85,16 @@ __global__ void fuse_step_kernel(FuseParams p) {
             }
         }
     }
-    const float dt = p.sigma_next - p.sigma;
-    const float in_scale = rsqrtf(p.sigma_next * p.sigma_next + 1.0f);
-    float4 l0 = *reinterpret_cast<float4*>(p.latents + (0 * HW + pix) * 4);
-    float4 l1 = *reinterpret_cast<float4*>(p.latents + (1 * HW + pix) * 4);
-    float e0[4], e1[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         e0[i] = u0[i] + p.guidance * (c0[i] - u0[i]);
         e1[i] = u1[i] + p.guidance * (c1[i] - u1[i]);
     }
-    l0.x += e0[0] * dt; l0.y += e0[1] * dt; l0.z += e0[2] * dt; l0.w += e0[3] * dt;
-    l1.x += e1[0] * dt; l1.y += e1[1] * dt; l1.z += e1[2] * dt; l1.w += e1[3] * dt;
+}
+
+// The new latents, their optional fp16 copy and the next step's scaled model inputs.
+__device__ __forceinline__ void store_step(const FuseParams& p, int pix, float4 l0, float4 l1, float in_scale) {
+    const size_t HW = p.HW;
     *reinterpret_cast<float4*>(p.latents + (0 * HW + pix) * 4) = l0;
     *reinterpret_cast<float4*>(p.latents + (1 * HW + pix) * 4) = l1;
     if (p.latents_f16) {
@@ -116,6 +126,58 @@ __global__ void fuse_step_kernel(FuseParams p) {
         o[0 * HW + pix] = s1;
         o[1 * HW + pix] = s1;
     }
+}
+
+__global__ void fuse_step_kernel(FuseParams p) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pix >= p.HW) return;
+    const size_t HW = p.HW;
+    float e0[4], e1[4];
+    fused_guided_eps(p, pix, e0, e1);
+    const float dt = p.sigma_next - p.sigma;
+    const float in_scale = rsqrtf(p.sigma_next * p.sigma_next + 1.0f);
+    float4 l0 = *reinterpret_cast<float4*>(p.latents + (0 * HW + pix) * 4);
+    float4 l1 = *reinterpret_cast<float4*>(p.latents + (1 * HW + pix) * 4);
+    // Euler on epsilon as x + eps * dt (the order omg_fuse_step has always rounded in)
+    l0.x += e0[0] * dt; l0.y += e0[1] * dt; l0.z += e0[2] * dt; l0.w += e0[3] * dt;
+    l1.x += e1[0] * dt; l1.y += e1[1] * dt; l1.z += e1[2] * dt; l1.w += e1[3] * dt;
+    store_step(p, pix, l0, l1, in_scale);
+}
+
+// x0 = c_x x + c_eps eps;  x' = a x + b x0 + c h + d z  for the four channels of one pixel of one image
+__device__ __forceinline__ float4 solver_update(const SolverParams& p, int img, int pix, float4 x, const float (&e)[4]) {
+    const size_t HW = p.f.HW;
+    float xs[4] = {x.x, x.y, x.z, x.w}, h[4] = {0.f, 0.f, 0.f, 0.f}, z[4] = {0.f, 0.f, 0.f, 0.f}, x0[4], o[4];
+    if (p.c != 0.f) {
+        const float4 hv = *reinterpret_cast<const float4*>(p.history + (img * HW + pix) * 4);
+        h[0] = hv.x; h[1] = hv.y; h[2] = hv.z; h[3] = hv.w;
+    }
+    if (p.d != 0.f) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) z[i] = __half2float(p.noise[(img * 4 + i) * HW + pix]);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        x0[i] = p.c_x * xs[i] + p.c_eps * e[i];
+        o[i] = p.a * xs[i] + p.b * x0[i] + p.c * h[i] + p.d * z[i];
+    }
+    if (p.store_x0) *reinterpret_cast<float4*>(p.history + (img * HW + pix) * 4) = make_float4(x0[0], x0[1], x0[2], x0[3]);
+    return make_float4(o[0], o[1], o[2], o[3]);
+}
+
+__global__ void solver_step_kernel(SolverParams p) {
+    griddep_launch_dependents();
+    griddep_wait();
+    const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pix >= p.f.HW) return;
+    const size_t HW = p.f.HW;
+    float e0[4], e1[4];
+    fused_guided_eps(p.f, pix, e0, e1);
+    const float4 l0 = *reinterpret_cast<const float4*>(p.f.latents + (0 * HW + pix) * 4);
+    const float4 l1 = *reinterpret_cast<const float4*>(p.f.latents + (1 * HW + pix) * 4);
+    store_step(p.f, pix, solver_update(p, 0, pix, l0, e0), solver_update(p, 1, pix, l1, e1), p.in_scale);
 }
 
 // out[b, w, :] = sum_n coef[w, n] * ctx[b, n, :]   (coef = M diag(alpha) or diag(1 - alpha); L = 77)
@@ -258,25 +320,24 @@ static int axpy_impl(const void* a, const void* b, float alpha, void* y, long lo
     return check_launch("axpy_kernel");
 }
 
-static int fuse_step_impl(const omg_fuse_desc* d, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    OMG_CHECK(d && d->noise_main && d->latents, "omg_fuse_step: null pointer");
-    OMG_CHECK(d->n_concepts >= 0 && d->n_concepts <= OMG_MAX_CONCEPTS, "omg_fuse_step: n_concepts=%d out of range",
+// Validates the fusion part of a step descriptor and fills p (who: the entry point named in errors).
+static int fuse_params(const omg_fuse_desc* d, const char* who, FuseParams& p) {
+    OMG_CHECK(d && d->noise_main && d->latents, "%s: null pointer", who);
+    OMG_CHECK(d->n_concepts >= 0 && d->n_concepts <= OMG_MAX_CONCEPTS, "%s: n_concepts=%d out of range", who,
               d->n_concepts);
-    OMG_CHECK(d->HW >= 1, "omg_fuse_step: empty latent");
-    if (check_aligned("omg_fuse_step", 16, {{"latents", d->latents}, {"next_main_in", d->next_main_in},
-                                            {"next_concept_in", d->next_concept_in}}) ||
-        check_aligned("omg_fuse_step", 8, {{"noise_main", d->noise_main}}) ||
-        check_aligned("omg_fuse_step", 4, {{"latents_f16", d->latents_f16}}))
+    OMG_CHECK(d->HW >= 1, "%s: empty latent", who);
+    if (check_aligned(who, 16, {{"latents", d->latents}, {"next_main_in", d->next_main_in},
+                                {"next_concept_in", d->next_concept_in}}) ||
+        check_aligned(who, 8, {{"noise_main", d->noise_main}}) ||
+        check_aligned(who, 4, {{"latents_f16", d->latents_f16}}))
         return 1;
-    FuseParams p;
     p.noise_main = static_cast<const __half*>(d->noise_main);
     for (int k = 0; k < OMG_MAX_CONCEPTS; ++k) {
         p.noise_concept[k] = k < d->n_concepts ? static_cast<const __half*>(d->noise_concept[k]) : nullptr;
         p.mask[k] = k < d->n_concepts ? static_cast<const float*>(d->mask[k]) : nullptr;
         OMG_CHECK(k >= d->n_concepts || p.mask[k] == nullptr || p.noise_concept[k] != nullptr,
-                  "omg_fuse_step: concept %d has a mask but no noise prediction", k);
-        if (check_aligned("omg_fuse_step", 8, {{"noise_concept", p.noise_concept[k]}})) return 1;
+                  "%s: concept %d has a mask but no noise prediction", who, k);
+        if (check_aligned(who, 8, {{"noise_concept", p.noise_concept[k]}})) return 1;
     }
     p.n_concepts = d->n_concepts;
     p.guidance = d->guidance;
@@ -287,8 +348,40 @@ static int fuse_step_impl(const omg_fuse_desc* d, void* stream_) {
     p.next_concept_in = static_cast<__half*>(d->next_concept_in);
     p.latents_f16 = static_cast<__half*>(d->latents_f16);
     p.HW = d->HW;
+    return 0;
+}
+
+static int fuse_step_impl(const omg_fuse_desc* d, void* stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    FuseParams p;
+    if (fuse_params(d, "omg_fuse_step", p)) return 1;
     OMG_CUDA(launch_pdl(fuse_step_kernel, dim3((d->HW + 127) / 128), dim3(128), 0, stream, p));
     return check_launch("fuse_step_kernel");
+}
+
+static int solver_step_impl(const omg_solver_desc* d, void* stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    OMG_CHECK(d, "omg_solver_step: null pointer");
+    SolverParams p;
+    if (fuse_params(&d->fuse, "omg_solver_step", p.f)) return 1;
+    OMG_CHECK(d->d == 0.f || d->noise, "omg_solver_step: d=%g needs noise", (double)d->d);
+    OMG_CHECK((d->c == 0.f && !d->store_x0) || d->history, "omg_solver_step: c=%g / store_x0=%d needs history",
+              (double)d->c, d->store_x0);
+    if (check_aligned("omg_solver_step", 16, {{"history", d->history}}) ||
+        check_aligned("omg_solver_step", 2, {{"noise", d->noise}}))
+        return 1;
+    p.c_x = d->c_x;
+    p.c_eps = d->c_eps;
+    p.a = d->a;
+    p.b = d->b;
+    p.c = d->c;
+    p.d = d->d;
+    p.in_scale = d->input_scale;
+    p.history = static_cast<float*>(d->history);
+    p.noise = static_cast<const __half*>(d->noise);
+    p.store_x0 = d->store_x0 != 0;
+    OMG_CUDA(launch_pdl(solver_step_kernel, dim3((d->fuse.HW + 127) / 128), dim3(128), 0, stream, p));
+    return check_launch("solver_step_kernel");
 }
 
 static int ctx_mix_impl(const void* ctx, const void* coef, void* out, int B, int L, int C, void* stream_) {
@@ -323,6 +416,15 @@ extern "C" int omg_fuse_step(const omg_fuse_desc* d, void* stream_) {
     if (rc == 0 && ::omg::plan_recording()) {
         const omg_fuse_desc c = *d;  // by value: a plan outlives the caller's descriptor
         ::omg::plan_note([c](void* s) { return fuse_step_impl(&c, s); });
+    }
+    return rc;
+}
+
+extern "C" int omg_solver_step(const omg_solver_desc* d, void* stream_) {
+    const int rc = solver_step_impl(d, stream_);
+    if (rc == 0 && ::omg::plan_recording()) {
+        const omg_solver_desc c = *d;
+        ::omg::plan_note([c](void* s) { return solver_step_impl(&c, s); });
     }
     return rc;
 }

@@ -507,9 +507,8 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     return out
 
 
-def fuse_step(noise_main, noise_concepts, masks, guidance, sigma, sigma_next, latents, next_main_in=None,
-              next_concept_in=None, latents_f16=None):
-    d = L.FuseDesc()
+def _fuse_desc(d, noise_main, noise_concepts, masks, guidance, sigma, sigma_next, latents, next_main_in,
+               next_concept_in, latents_f16):
     d.noise_main = noise_main.data_ptr()
     d.n_concepts = len(noise_concepts)
     for i, (n, m) in enumerate(zip(noise_concepts, masks)):
@@ -521,7 +520,35 @@ def fuse_step(noise_main, noise_concepts, masks, guidance, sigma, sigma_next, la
     d.next_concept_in = _ptr(next_concept_in)
     d.latents_f16 = _ptr(latents_f16)
     d.HW = latents.shape[1] * latents.shape[2] if latents.dim() == 4 else latents.shape[1]
+
+
+def fuse_step(noise_main, noise_concepts, masks, guidance, sigma, sigma_next, latents, next_main_in=None,
+              next_concept_in=None, latents_f16=None):
+    d = L.FuseDesc()
+    _fuse_desc(d, noise_main, noise_concepts, masks, guidance, sigma, sigma_next, latents, next_main_in,
+               next_concept_in, latents_f16)
     L.check(L.load().omg_fuse_step(C.byref(d), _stream()), "omg_fuse_step")
+
+
+def solver_step(noise_main, noise_concepts, masks, guidance, coeffs, latents, next_main_in=None, next_concept_in=None,
+                latents_f16=None, history=None, store_x0=False, noise=None):
+    """omg_fuse_step's fusion and guidance with the update of `coeffs` (omg_b200.scheduler.StepCoeffs):
+    x0 = c_x x + c_eps eps, x' = a x + b x0 + c history + d noise, next inputs = x' * s.  history: fp32 (2, h, w, 4),
+    overwritten with x0 when store_x0; noise: fp16 (2, 4, h, w) as torch.randn draws it."""
+    d = L.SolverDesc()
+    _fuse_desc(d.fuse, noise_main, noise_concepts, masks, guidance, 0.0, 0.0, latents, next_main_in, next_concept_in,
+               latents_f16)
+    d.c_x, d.c_eps, d.a, d.b, d.c, d.d, d.input_scale = (float(v) for v in coeffs)
+    if history is not None and (history.dtype != torch.float32 or not history.is_contiguous()
+                                or history.numel() != 2 * d.fuse.HW * 4):
+        raise ValueError("history must be a contiguous fp32 (2, h, w, 4) tensor")
+    if noise is not None and (noise.dtype != torch.float16 or not noise.is_contiguous()
+                              or noise.numel() != 2 * 4 * d.fuse.HW):
+        raise ValueError("noise must be a contiguous fp16 (2, 4, h, w) tensor")
+    d.history = _ptr(history)
+    d.noise = _ptr(noise)
+    d.store_x0 = int(bool(store_x0))
+    L.check(L.load().omg_solver_step(C.byref(d), _stream()), "omg_solver_step")
 
 
 def axpy(a, b, alpha=1.0, out=None):

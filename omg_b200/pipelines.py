@@ -13,7 +13,9 @@ VAE, segmentation and face analysis sit outside the hot path (SURVEY section 8):
 by a pluggable `prompt_encoder`, `output_type="latent"` is native and image output needs a `vae_decoder`.
 
 Per step (one iteration of lora_pipeline.py:485-632) the device executes: main UNet (CUDA graph) -> [concept
-UNets (CUDA graphs)] -> omg_fuse_step.  No host sync happens inside the loop.
+UNets (CUDA graphs)] -> omg_fuse_step (Euler on epsilon) or omg_solver_step (every other schedule of
+omg_b200.scheduler).  No host sync happens inside the loop.  `pipe.scheduler` is any schedule of omg_b200.scheduler;
+`from_pretrained` reads the checkpoint's scheduler/scheduler_config.json.
 """
 import hashlib
 import os
@@ -26,7 +28,7 @@ import torch
 from . import ops
 from .config import UNetConfig
 from .prompt_attention import AttentionReplace
-from .scheduler import EulerDiscreteSchedule
+from .scheduler import EulerDiscreteSchedule, _Schedule, load_scheduler
 from .unet import PackedUNet, UNetRunner
 
 FUSION_AFTER_STEP = 15  # `if i > 15 and stage == 2` (lora_pipeline.py:568)
@@ -223,6 +225,7 @@ class _BasePipeline:
         if isinstance(controlnet, (str, os.PathLike)):
             controlnet = load_controlnet(controlnet, device)
         pipe = cls(unet, controlnet=controlnet, prompt_encoder=prompt_encoder, vae_decoder=vae_decoder, use_graphs=use_graphs)
+        pipe.scheduler = load_scheduler(pretrained_model)
         return pipe
 
     def to(self, device=None, *_, **__):
@@ -332,27 +335,37 @@ class _BasePipeline:
             for r in runners:
                 r.update_context_rows(4, rows)
 
+    def _set_timesteps(self, num_inference_steps: int):
+        if not isinstance(self.scheduler, _Schedule):
+            raise ValueError(f"pipe.scheduler: {type(self.scheduler).__name__} is not supported; use a schedule of "
+                             "omg_b200.scheduler (EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, "
+                             "DPMSolverMultistepScheduler)")
+        return self.scheduler.set_timesteps(num_inference_steps)
+
     def _step_end(self, callback, i, t, lat, main, cbuf):
         """`callback_on_step_end(self, i, t, {"latents": latents})` (lora_pipeline.py:617-625): the callback sees the
-        latents after the scheduler step as (2,4,h,w) and may return {"latents": replacement}."""
+        latents after the scheduler step as (2,4,h,w) and may return {"latents": replacement}.  A multistep schedule's
+        history (the previous x0) is left as it is, as diffusers' scheduler keeps its own."""
         view = lat.permute(0, 3, 1, 2)
         given = view.clone()
         out = callback(self, i, t, {"latents": given})
         new = (out or {}).get("latents", given)
         if new is not given:
             lat.copy_(new.to(lat.device, lat.dtype).permute(0, 2, 3, 1))
-            if i + 1 < len(self.scheduler.sigmas) - 1:  # next step's scaled inputs (fuse_step wrote them from the old latents)
+            if i + 1 < len(self.scheduler.timesteps):  # next step's scaled inputs (the step wrote them from the old latents)
                 x = (lat * self.scheduler.input_scale(i + 1)).half()
                 main.sample_in[..., :4] = torch.cat([x, x], dim=0)
                 cbuf[..., :4] = torch.cat([x[1:2], x[1:2]], dim=0)
 
     def _denoise(self, *, ts, lat, ctx4, pooled4, tid, concepts, masks, stage, guidance_scale, h, w, concept_unet,
-                 main_cn=None, identity=None, callback=None):
+                 main_cn=None, identity=None, callback=None, generator=None):
         """The step loop (lora_pipeline.py:485-632 / instantid_pipeline.py:540-690).
 
         concepts: list of dicts {ctx (2, L, D) [text tokens (+ IP tokens)], pooled (2, P), lora_key, ip (bool)};
         main_cn:  None or (ControlNet PackedUNet, condition image (4,3,H,W), scale, keep(i) -> 0/1) for the main rows;
-        identity: None or (IdentityNet PackedUNet, condition image (2,3,H,W), scale, [face tokens (2,16,D) per concept]).
+        identity: None or (IdentityNet PackedUNet, condition image (2,3,H,W), scale, [face tokens (2,16,D) per concept]);
+        generator: the call's generator; a stochastic schedule draws its per-step noise from it as diffusers'
+                   randn_tensor does (on the generator's device; torch's global CUDA RNG when None).
 
         Steps without fusion run the main UNet alone (B=4).  Fusion steps (index > 15, stage 2) run ONE grouped
         forward: rows 0-3 = main stream, then two rows per active concept, every stream with its own LoRA segment /
@@ -360,7 +373,8 @@ class _BasePipeline:
         (the reference's two pipelines load the same checkpoint, inference_lora.py:153-159); otherwise the concept
         streams run as separate forwards."""
         dev = self._execution_device
-        sig = self.scheduler.sigmas
+        sch = self.scheduler
+        sig = sch.sigmas
         controller = self.controller
         active = [k for k in range(len(concepts)) if stage == 2 and masks[k] is not None]
         n_act = len(active)
@@ -418,20 +432,43 @@ class _BasePipeline:
         #  * twin rows: until the first fusion step image 1 IS image 0 (same latents, same prompt, and the
         #    prompt-to-prompt edit of identical rows is the identity), so the main UNet runs B=2 [uncond, cond];
         #  * stage-2 prefix: steps 0..15 of stage 2 repeat stage 1 on the same inputs, so stage 2 resumes from the
-        #    latents stage 1 had after step 15.
+        #    latents stage 1 had after step 15 (and the solver history and generator state it had then).  A stochastic
+        #    schedule gives the two images different noise (no twins), and without a generator its noise comes from
+        #    the global RNG, which cannot be replayed (no prefix).
+        hist = torch.zeros((2, h, w, 4), dtype=torch.float32, device=dev) if sch.uses_history else None
+        gdev = generator.device if generator is not None else dev
+
+        def step(noise_main, noises, fmasks, i):
+            if sch.uses_fuse_step:
+                ops.fuse_step(noise_main, noises, fmasks, guidance_scale, float(sig[i]), float(sig[i + 1]), lat,
+                              main.sample_in, cbuf)
+                return
+            z = None
+            if sch.stochastic:  # randn_tensor(model_output.shape, generator, device, fp16)
+                z = torch.randn((2, 4, h, w), generator=generator, device=gdev, dtype=torch.float16).to(dev)
+            ops.solver_step(noise_main, noises, fmasks, guidance_scale, sch.step_coeffs(i), lat, main.sample_in, cbuf,
+                            history=hist, store_x0=hist is not None, noise=z)
+
         dd = self.dedup and cn is None
-        twin = dd and bool(torch.equal(lat[0], lat[1]) and torch.equal(ctx4[0], ctx4[1]) and torch.equal(ctx4[2], ctx4[3])
+        prefix_ok = dd and not (sch.stochastic and generator is None)
+        gen0 = generator.get_state() if (sch.stochastic and generator is not None) else None
+        twin = dd and not sch.stochastic and bool(torch.equal(lat[0], lat[1]) and torch.equal(ctx4[0], ctx4[1]) and torch.equal(ctx4[2], ctx4[3])
                            and torch.equal(pooled4[0], pooled4[1]) and torch.equal(pooled4[2], pooled4[3]))
         i0 = 0
-        sig_key = (tuple(float(t) for t in ts), float(guidance_scale), self.main_lora_key, h, w)
-        if dd and stage == 2 and n_act > 0 and len(ts) > FUSION_AFTER_STEP + 1 and self._prefix is not None:
+        sig_key = (tuple(float(t) for t in ts), float(guidance_scale), self.main_lora_key, h, w, sch.scheduler_key())
+        if prefix_ok and stage == 2 and n_act > 0 and len(ts) > FUSION_AFTER_STEP + 1 and self._prefix is not None:
             pf = self._prefix
             if (pf["key"] == sig_key and torch.equal(pf["lat0"], lat) and torch.equal(pf["ctx4"], ctx4.to(dev))
-                    and torch.equal(pf["pooled4"], pooled4.to(dev))):
+                    and torch.equal(pf["pooled4"], pooled4.to(dev))
+                    and (gen0 is None or (pf["gen0"] is not None and torch.equal(pf["gen0"], gen0)))):
                 i0 = FUSION_AFTER_STEP + 1
                 lat.copy_(pf["lat"])
                 main.sample_in.copy_(pf["sample_in"])
                 cbuf.copy_(pf["cbuf"])
+                if hist is not None:
+                    hist.copy_(pf["hist"])
+                if gen0 is not None:
+                    generator.set_state(pf["gen"])
                 if controller is not None:
                     for _ in range(i0):
                         controller.advance(n_att)
@@ -441,7 +478,15 @@ class _BasePipeline:
             main2 = self._runner("main2", self.unet, 2, h, w, groups=[RowGroup(0, 2, self.main_lora_key, False)])
             main2.set_conditioning(ts, ctx4[[0, 2]], pooled4[[0, 2]], tid.repeat(2, 1))
             noise4 = torch.empty((4, h, w, 8), dtype=torch.float16, device=dev)
-        lat0_keep = lat.clone() if (dd and stage == 1) else None
+        lat0_keep = lat.clone() if (prefix_ok and stage == 1) else None
+
+        def keep_prefix():
+            self._prefix = {"key": sig_key, "lat0": lat0_keep, "ctx4": ctx4.to(dev).clone(),
+                            "pooled4": pooled4.to(dev).clone(), "lat": lat.clone(),
+                            "sample_in": main.sample_in.clone(), "cbuf": cbuf.clone(),
+                            "hist": None if hist is None else hist.clone(), "gen0": gen0,
+                            "gen": None if gen0 is None else generator.get_state()}
+
         for i in range(i0, len(ts)):
             fuse = i > FUSION_AFTER_STEP and n_act > 0
             if twin and not fuse:
@@ -451,13 +496,11 @@ class _BasePipeline:
                 if controller is not None:
                     controller.advance(n_att)
                 self.sample_forwards += 2
-                ops.fuse_step(noise4, [], [], guidance_scale, float(sig[i]), float(sig[i + 1]), lat, main.sample_in, cbuf)
+                step(noise4, [], [], i)
                 if callback is not None:
                     self._step_end(callback, i, ts[i], lat, main, cbuf)
                 if lat0_keep is not None and i == FUSION_AFTER_STEP:
-                    self._prefix = {"key": sig_key, "lat0": lat0_keep, "ctx4": ctx4.to(dev).clone(),
-                                    "pooled4": pooled4.to(dev).clone(), "lat": lat.clone(),
-                                    "sample_in": main.sample_in.clone(), "cbuf": cbuf.clone()}
+                    keep_prefix()
                 continue
             twin = False  # from the first fusion step on the two images differ
             if controller is not None:
@@ -516,14 +559,11 @@ class _BasePipeline:
                         noises.append(r.forward(i, v, key=ckey))
                 fmasks = [masks[k] for k in active]
             self.sample_forwards += 4 + (2 * n_act if fuse else 0)
-            ops.fuse_step(noise[0:4] if run is fused else noise, noises, fmasks, guidance_scale, float(sig[i]),
-                          float(sig[i + 1]), lat, main.sample_in, cbuf)
+            step(noise[0:4] if run is fused else noise, noises, fmasks, i)
             if callback is not None:
                 self._step_end(callback, i, ts[i], lat, main, cbuf)
             if lat0_keep is not None and i == FUSION_AFTER_STEP:
-                self._prefix = {"key": sig_key, "lat0": lat0_keep, "ctx4": ctx4.to(dev).clone(),
-                                "pooled4": pooled4.to(dev).clone(), "lat": lat.clone(),
-                                "sample_in": main.sample_in.clone(), "cbuf": cbuf.clone()}
+                keep_prefix()
         return lat
 
     def _finish(self, latents_nhwc: torch.Tensor, output_type: str, return_dict: bool):
@@ -580,8 +620,7 @@ class LoraMultiConceptPipeline(_BasePipeline):
         if stage == 2:
             masks = [_binary_latent_mask(m, h, w, dev) for m in region_masks]
         # 5/6 timesteps + latents
-        ts = self.scheduler.set_timesteps(num_inference_steps)
-        sig = self.scheduler.sigmas
+        ts = self._set_timesteps(num_inference_steps)
         lat = self.prepare_latents(h, w, generator, latents)
         # 7.2 added conditioning
         original_size = original_size or (height, width)
@@ -603,7 +642,8 @@ class LoraMultiConceptPipeline(_BasePipeline):
             c["ip"] = False
         lat = self._denoise(ts=ts, lat=lat, ctx4=ctx4, pooled4=pooled4, tid=tid, concepts=concepts, masks=masks,
                             stage=stage, guidance_scale=guidance_scale, h=h, w=w, concept_unet=concept_models.unet
-                            if concept_models is not None else self.unet, main_cn=main_cn, callback=callback_on_step_end)
+                            if concept_models is not None else self.unet, main_cn=main_cn, callback=callback_on_step_end,
+                            generator=generator)
         return self._finish(lat, output_type, return_dict)
 
     def _prepare_image(self, image, width, height, batch):
@@ -671,8 +711,7 @@ class InstantidMultiConceptPipeline(_BasePipeline):
         masks = [None] * len(concepts)
         if stage == 2:
             masks = [_binary_latent_mask(m, h, w, dev) for m in region_masks]
-        ts = self.scheduler.set_timesteps(num_inference_steps)
-        sig = self.scheduler.sigmas
+        ts = self._set_timesteps(num_inference_steps)
         lat = self.prepare_latents(h, w, generator, latents)
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
@@ -697,7 +736,7 @@ class InstantidMultiConceptPipeline(_BasePipeline):
         lat = self._denoise(ts=ts, lat=lat, ctx4=ctx4, pooled4=pooled4, tid=tid, concepts=concepts, masks=masks,
                             stage=stage, guidance_scale=guidance_scale, h=h, w=w, concept_unet=concept_models.unet
                             if concept_models is not None else self.unet, main_cn=main_cn, identity=identity,
-                            callback=callback_on_step_end)
+                            callback=callback_on_step_end, generator=generator)
         return self._finish(lat, output_type, return_dict)
 
     def get_face_embedding(self, face_app, ref_image):
