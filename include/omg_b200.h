@@ -404,6 +404,70 @@ typedef struct {
 
 int omg_scrfd_detect(const omg_scrfd_desc* desc, void* stream);
 
+/*
+ * YOLO-World (ultralytics WorldModel: the open-vocabulary detector whose boxes prompt SAM between OMG's two stages).
+ * Its convolutions and linears run on omg_gemm, SPPF's max-pool on omg_pool2d, up-sampling on omg_channel_op,
+ * LayerNorm on omg_layernorm and the pooling attention on omg_attention_small; these are the ops that are not.
+ *
+ * omg_text_gate: MaxSigmoidAttnBlock after its convs, fp32 arithmetic, per image b and pixel of a B x HW grid:
+ *   gate[h] = sigmoid(max_k <embed[b, pix, h*hc : (h+1)*hc], guide[b, k, h*hc : (h+1)*hc]> / sqrt(hc) + bias[h])
+ *             * scale[h]                                        (hc = Ce / nh; scale NULL = 1)
+ *   out[b, pix, c] = p[b, pix, c] * gate[c / (C2 / nh)]
+ * embed fp16 rows of ld_e elements (Ce channels), guide fp32 [B, n, Ce] contiguous (gl(text) of each image, so images
+ * with different prompts share one launch), bias / scale fp32 [nh], p (proj_conv's output) and out fp16 rows of ld_p /
+ * ld_o elements (C2 channels; out may alias p - the gated slice of C2fAttn's concat buffer).  n >= 1, hc 16 | 32 | 64,
+ * C2 % nh == 0, C2 and every row stride a multiple of 8, embed / p / out 16 B aligned; the guide of one image
+ * (n * Ce floats) must fit in shared memory.
+ * omg_adaptive_maxpool: AdaptiveMaxPool2d((k, k)) of x [B, H, W, C] (rows of ldx elements) with PyTorch's windows
+ *   [floor(i H / k), ceil((i + 1) H / k)) (overlapping when k does not divide H); patch i * k + j of image b goes to
+ *   out + b * out_bs + (row0 + i * k + j) * out_ld (fp16, C channels): ImagePoolingAttn's 3 levels x 9 patches fill
+ *   rows 0..26 of its key buffer.  C, ldx, out_ld and out_bs multiples of 8, x / out 16 B aligned.
+ * omg_yolo_detect: WorldDetect + non_max_suppression + scale_boxes for one image, in up to two launches.
+ *   (a) one warp per anchor over the levels (row-major grids, anchor centre (x + 0.5, y + 0.5) * stride):
+ *       logit_k = <x', text[k]> * cls_scale[l] + cls_bias[l] with x' = x / max(|x|, 1e-12) when normalize_x (the
+ *       plain ContrastiveHead; BNContrastiveHead's BatchNorm is folded into the embedding conv instead and
+ *       normalize_x = 0), text [nc, E] fp32 already L2-normalised, cls_scale = exp(logit_scale); score = max_k
+ *       sigmoid(logit_k), cls = its first argmax; DFL (softmax expectation over 16 bins of each side's box logits) and
+ *       dist2bbox -> xywh -> xyxy in letterbox pixels.  rows [T, 6] fp32 = [x0, y0, x1, y1, score, cls] per anchor.
+ *   (b) skipped when out is NULL; otherwise one CTA: anchors with score > conf (strict), a descending sort (ties: lower
+ *       anchor index first), greedy NMS on boxes offset by cls * max_wh (0 when agnostic) that suppresses IoU > iou
+ *       (torchvision's IoU, no +1), at most max_det rows, then (box - pad) / gain clipped to [0, clip_w] x [0, clip_h],
+ *       all fp32 without contraction.  out [max_out, 6] rows [x0, y0, x1, y1, score, cls]; *count (device int).
+ *   box: fp16 rows of box_ld elements, the 4 x 16 DFL logits (l, t, r, b); emb: fp16 rows of emb_ld elements, E channels.
+ *   At most OMG_YOLO_MAX_ANCHORS anchors (640 x 640 at strides 8 / 16 / 32 is 8 400) and OMG_YOLO_MAX_CLASSES classes.
+ *   Cost of (b): the rank of each of the n candidates is a count over all n (n^2 shared-memory reads over 1024
+ *   threads), then one barrier per kept row.  ultralytics' max_nms (30 000) never binds below the anchor cap, so n is
+ *   every anchor above conf: at most 17 800 (about 310 000 reads per thread).
+ */
+int omg_text_gate(const void* embed, long long ld_e, int Ce, const float* guide, int n, const float* bias,
+                  const float* scale, int nh, const void* p, long long ld_p, void* out, long long ld_o, int C2, int B,
+                  int HW, void* stream);
+int omg_adaptive_maxpool(const void* x, long long ldx, int B, int H, int W, int C, int k, void* out, long long out_bs,
+                         long long out_ld, int row0, void* stream);
+
+#define OMG_YOLO_MAX_LEVELS 4
+#define OMG_YOLO_MAX_ANCHORS 17800
+#define OMG_YOLO_MAX_CLASSES 1024
+#define OMG_YOLO_REG_MAX 16
+typedef struct {
+    const void* box[OMG_YOLO_MAX_LEVELS];
+    const void* emb[OMG_YOLO_MAX_LEVELS];
+    int64_t box_ld[OMG_YOLO_MAX_LEVELS], emb_ld[OMG_YOLO_MAX_LEVELS];
+    float cls_scale[OMG_YOLO_MAX_LEVELS], cls_bias[OMG_YOLO_MAX_LEVELS];
+    int32_t stride[OMG_YOLO_MAX_LEVELS], fh[OMG_YOLO_MAX_LEVELS], fw[OMG_YOLO_MAX_LEVELS];
+    int32_t n_levels, nc, E, normalize_x;
+    const float* text;   /* [nc, E] */
+    float* rows;         /* [anchors, 6] */
+    float conf, iou, max_wh;
+    int32_t agnostic, max_det;
+    float gain, pad_x, pad_y, clip_w, clip_h;
+    float* out;          /* [max_out, 6], or NULL: pass (a) only */
+    int32_t max_out;
+    int32_t* count;      /* device */
+} omg_yolo_desc;
+
+int omg_yolo_detect(const omg_yolo_desc* desc, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Launch plans: a forward as a handle.  The reference drives one UNet forward as a Python call
  * (`self.unet(latent_model_input, t, ...)`, src/pipelines/lora_pipeline.py:558-567, 588-606); a host that is not Python -

@@ -2,7 +2,7 @@
 """OMG + InstantID multi-identity generation on the H100 path.  The reference CLI's flags (names, defaults, types:
 inference_instantid.py:259-286, pinned by tests/golden/cli_flags.json), prompt mini-DSL, two-stage flow and output
 files; additions (non-breaking): --synthetic, --tiny, --num_inference_steps, --image_size, --dedup, --mask_boxes,
---face_embeds, --face_kps, --sam_boxes, --decode.
+--face_embeds, --face_kps, --sam_boxes, --decode, --detect (with --yoloworld_checkpoint, --clip_checkpoint).
 
 Face analysis: insightface's FaceAnalysis('antelopev2') when `insightface` is importable; otherwise, when
 <antelopev2_path>/models/antelopev2/ holds scrfd_10g_bnkps.onnx and glintr100.onnx, omg_b200.face.FaceAnalysis runs the
@@ -19,7 +19,8 @@ Output: with --decode the VAE decodes both stages to stage-1.png / stage-2.png a
 checkpoint's own VAE (<pretrained_model>/vae) in bf16, whose exponent range holds activations that overflow fp16 with
 SDXL's VAE weights, or a random-init VAE with --synthetic.  Then --sam_boxes (EfficientViT-SAM masks from box prompts on
 the decoded stage-1 image, see inference_lora.py) replaces the stage-2 region masks.  Without --decode the latents are
-saved (stage-{1,2}.pt) and --sam_boxes is refused.
+saved (stage-{1,2}.pt) and --sam_boxes is refused.  --detect finds those boxes with YOLO-World instead (the best box
+of "man" and of "woman" when in the prompt, see inference_lora.py); the key-points then come from the stage-1 image.
 """
 import argparse
 import math
@@ -111,6 +112,12 @@ def parse_args():
     p.add_argument("--mask_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (pixels), replaces segmentation")
     p.add_argument("--sam_boxes", default="", type=str, help="x0,y0,x1,y1|... box prompts for EfficientViT-SAM on the "
                    "decoded stage-1 image (needs a decoded image; excludes --mask_boxes)")
+    p.add_argument("--detect", action="store_true", help="find 'man' / 'woman' (when in the prompt) in the decoded "
+                   "stage-1 image with YOLO-World; the best boxes prompt SAM; needs --decode, excludes --mask_boxes "
+                   "and --sam_boxes")
+    p.add_argument("--yoloworld_checkpoint", default="./checkpoint/yolo_world/l/yolo-world.pt", type=str)
+    p.add_argument("--clip_checkpoint", default="./checkpoint/clip/ViT-B-32.pt", type=str,
+                   help="CLIP ViT-B/32 for YOLO-World's class embeddings: OpenAI's ViT-B-32.pt or an HF directory")
     p.add_argument("--decode", action="store_true", help="decode to PNG: <pretrained_model>/vae in bf16 (with "
                    "--synthetic: a random-init VAE decoder)")
     p.add_argument("--face_embeds", default="", type=str, help="a.pt|b.pt: 512-d identity embeddings, one per region "
@@ -295,6 +302,10 @@ if __name__ == "__main__":
     decoded = pipe.vae_decoder is not None
     from omg_b200 import sam as sam_lib
     sam_lib.check_sam_flags(args.sam_boxes, args.mask_boxes, decoded=decoded)
+    from omg_b200 import yolo_world
+    yolo_world.check_detect_flags(args.detect, args.segment_type, args.mask_boxes, args.sam_boxes, decoded)
+    if args.detect and len(regions) != len(yolo_world.DETECT_WORDS):
+        raise SystemExit(f"--detect finds {' and '.join(yolo_world.DETECT_WORDS)}: it needs 2 regions, not {len(regions)}")
     sam_boxes = None
     if args.sam_boxes:
         try:
@@ -309,6 +320,12 @@ if __name__ == "__main__":
                   guidance_scale=args.cfg_scale, face_embeds=faces, **kwargs)
     image = sample_image(pipe, generator=torch.Generator(device).manual_seed(args.seed), stage=1, **common)
     controller.reset()
+    if args.detect:
+        # the YOLO-World branch of predict_mask (inference_instantid.py:158-193,341-349): the best box of each word
+        tok = yolo_world.WordTokenizer() if args.synthetic else pipe.tokenizer
+        detector = yolo_world.make_detector(args.synthetic, args.tiny, args.yoloworld_checkpoint, args.clip_checkpoint,
+                                            tok, device)
+        sam_boxes = yolo_world.detect_boxes(detector, image[0], args.prompt, tok)
     if sam_boxes is not None:
         # predict_mask (inference_lora.py:91-126) with the boxes as the detections, on the decoded stage-1 image:
         # --segment_type GroundingDINO prompts the original SAM (ViT-H, --sam_checkpoint), any other value

@@ -1,13 +1,15 @@
 #!/usr/bin/env python
 """OMG + LoRA multi-concept generation on the H100 path.  Same flags, prompt mini-DSL, two-stage flow and output
 files as the reference CLI (inference_lora.py:201-323); additions (non-breaking): --synthetic, --num_inference_steps,
---image_size, --mask_boxes, --vae_fp16_safe, --sam_boxes.
+--image_size, --mask_boxes, --vae_fp16_safe, --sam_boxes, --detect (with --yoloworld_checkpoint, --clip_checkpoint).
 
 Masks between the stages: with --sam_boxes (x0,y0,x1,y1 per concept, '|' separated, stage-1 pixels) the boxes prompt
 EfficientViT-SAM xl1 on the decoded stage-1 image, as the reference's predict_mask does with a detector's box
 (inference_lora.py:91-126), and the device masks go straight into stage 2 (weights from --efficientViT_checkpoint, or
-random with --synthetic; needs a decoded image: --decode or --vae_fp16_safe).  The detectors (YOLO-World /
-GroundingDINO) stay outside: boxes are an input.  --mask_boxes instead fills the boxes as rectangles; in --synthetic mode
+random with --synthetic; needs a decoded image: --decode or --vae_fp16_safe).  --detect finds those boxes itself, as
+the reference's default `--segment_type yoloworld` does: YOLO-World (omg_b200/yolo_world.py, CLIP ViT-B/32 class
+embeddings) takes the best box of "man" and of "woman" when the word is among the prompt's tokens.  The GroundingDINO
+detector is not built: with `--segment_type GroundingDINO` the boxes stay an input.  --mask_boxes instead fills the boxes as rectangles; in --synthetic mode
 without either flag the masks are the fixed config-2 rectangles.
 
 Output: with --decode the checkpoint's own VAE (<pretrained_sdxl_model>/vae, the original SDXL weights) decodes in bf16,
@@ -90,6 +92,12 @@ def parse_args():
     p.add_argument("--sam_boxes", default="", type=str, help="x0,y0,x1,y1|x0,y0,x1,y1 (stage-1 pixels, one per concept, "
                    "empty = skip the concept): box prompts for EfficientViT-SAM on the decoded stage-1 image, whose masks "
                    "drive stage 2; needs a decoded image, excludes --mask_boxes")
+    p.add_argument("--detect", action="store_true", help="find 'man' / 'woman' (when in the prompt) in the decoded "
+                   "stage-1 image with YOLO-World; the best boxes prompt SAM; needs a decoded image, excludes "
+                   "--mask_boxes and --sam_boxes")
+    p.add_argument("--yoloworld_checkpoint", default="./checkpoint/yolo_world/l/yolo-world.pt", type=str)
+    p.add_argument("--clip_checkpoint", default="./checkpoint/clip/ViT-B-32.pt", type=str,
+                   help="CLIP ViT-B/32 for YOLO-World's class embeddings: OpenAI's ViT-B-32.pt or an HF directory")
     return p.parse_args()
 
 
@@ -163,7 +171,7 @@ def build_model_sd(args, prompts, device):
         adapter_name = lora_path.split("/")[-1].split(".")[0]
         pipe_concept.load_lora_weights(lora_path, weight_name="pytorch_lora_weights.safetensors", adapter_name=adapter_name)
         pipe_list.append(adapter_name)
-    if not args.mask_boxes:
+    if not (args.mask_boxes or args.sam_boxes or args.detect):
         print("no --mask_boxes given: only stage 1 (the layout pass) will run")
     return pipe, controller, pipe_concept, pipe_list, [None] * len(pipe_list)
 
@@ -201,6 +209,10 @@ if __name__ == "__main__":
     decoded = pipe.vae_decoder is not None
     from omg_b200 import sam as sam_lib
     sam_lib.check_sam_flags(args.sam_boxes, args.mask_boxes, decoded)
+    from omg_b200 import yolo_world
+    yolo_world.check_detect_flags(args.detect, args.segment_type, args.mask_boxes, args.sam_boxes, decoded)
+    if args.detect and len(pipe_list) != len(yolo_world.DETECT_WORDS):
+        raise SystemExit(f"--detect finds {' and '.join(yolo_world.DETECT_WORDS)}: it needs 2 concepts, not {len(pipe_list)}")
     sam_boxes = None
     if args.sam_boxes:
         try:
@@ -218,6 +230,12 @@ if __name__ == "__main__":
                   lora_list=pipe_list, styleL=styleL, num_inference_steps=args.num_inference_steps, **kwargs)
     image = sample_image(pipe, generator=torch.Generator(device).manual_seed(args.seed), stage=1, **common)
     controller.reset()
+    if args.detect:
+        # predict_mask's YOLO-World branch (inference_lora.py:109-116,275-283): the best box of each word of the prompt
+        tok = yolo_world.WordTokenizer() if args.synthetic else pipe.tokenizer
+        detector = yolo_world.make_detector(args.synthetic, args.tiny, args.yoloworld_checkpoint, args.clip_checkpoint,
+                                            tok, device)
+        sam_boxes = yolo_world.detect_boxes(detector, image[0], args.prompt, tok)
     if args.mask_boxes:
         masks = []
         for box in args.mask_boxes.split("|"):

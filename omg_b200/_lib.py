@@ -74,6 +74,23 @@ class ScrfdDesc(C.Structure):
                 ("count", C.c_void_p)]
 
 
+OMG_YOLO_MAX_LEVELS = 4
+OMG_YOLO_MAX_ANCHORS = 17800
+OMG_YOLO_MAX_CLASSES = 1024
+
+
+class YoloDesc(C.Structure):
+    _fields_ = [("box", C.c_void_p * OMG_YOLO_MAX_LEVELS), ("emb", C.c_void_p * OMG_YOLO_MAX_LEVELS),
+                ("box_ld", C.c_int64 * OMG_YOLO_MAX_LEVELS), ("emb_ld", C.c_int64 * OMG_YOLO_MAX_LEVELS),
+                ("cls_scale", C.c_float * OMG_YOLO_MAX_LEVELS), ("cls_bias", C.c_float * OMG_YOLO_MAX_LEVELS),
+                ("stride", C.c_int32 * OMG_YOLO_MAX_LEVELS), ("fh", C.c_int32 * OMG_YOLO_MAX_LEVELS),
+                ("fw", C.c_int32 * OMG_YOLO_MAX_LEVELS), ("n_levels", C.c_int32), ("nc", C.c_int32), ("E", C.c_int32),
+                ("normalize_x", C.c_int32), ("text", C.c_void_p), ("rows", C.c_void_p), ("conf", C.c_float),
+                ("iou", C.c_float), ("max_wh", C.c_float), ("agnostic", C.c_int32), ("max_det", C.c_int32),
+                ("gain", C.c_float), ("pad_x", C.c_float), ("pad_y", C.c_float), ("clip_w", C.c_float),
+                ("clip_h", C.c_float), ("out", C.c_void_p), ("max_out", C.c_int32), ("count", C.c_void_p)]
+
+
 class FuseDesc(C.Structure):
     _fields_ = [("noise_main", C.c_void_p), ("noise_concept", C.c_void_p * OMG_MAX_CONCEPTS),
                 ("mask", C.c_void_p * OMG_MAX_CONCEPTS), ("n_concepts", C.c_int32), ("guidance", C.c_float),
@@ -127,6 +144,11 @@ SYMBOLS = {
     "omg_pool2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                              C.c_int, C.c_int, C.c_void_p]),
     "omg_scrfd_detect": (C.c_int, [C.POINTER(ScrfdDesc), C.c_void_p]),
+    "omg_text_gate": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "omg_adaptive_maxpool": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                       C.c_longlong, C.c_longlong, C.c_int, C.c_void_p]),
+    "omg_yolo_detect": (C.c_int, [C.POINTER(YoloDesc), C.c_void_p]),
     "omg_plan_create": (C.c_void_p, []),
     "omg_plan_destroy": (None, [C.c_void_p]),
     "omg_plan_record_begin": (C.c_int, [C.c_void_p]),

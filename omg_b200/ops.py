@@ -662,6 +662,76 @@ def scrfd_detect(levels, num_anchors, det_thresh, det_scale, nms_thresh=0.4):
     return out[: int(count.item())]
 
 
+def text_gate(embed, guide, bias, nh, p, scale=None, out=None):
+    """omg_text_gate (MaxSigmoidAttnBlock's gating): embed (B, H, W, Ce) and p (B, H, W, C2) fp16 views with row-major
+    pixels (rows may be strided along the channel axis), guide fp32 (B, n, Ce), bias / scale fp32 [nh].  out (default:
+    p, in place) receives p * gate."""
+    _chk16(embed)
+    _chk16(p)
+    B, H, W, ld_e = _rows(embed)
+    _, _, _, ld_p = _rows(p)
+    out = p if out is None else out
+    _chk16(out)
+    _, _, _, ld_o = _rows(out)
+    assert p.shape[:3] == embed.shape[:3] == out.shape[:3] and out.shape[3] == p.shape[3]
+    Ce, C2 = embed.shape[3], p.shape[3]
+    for v in (guide, bias, scale):
+        assert v is None or (v.is_cuda and v.dtype == torch.float32 and v.is_contiguous())
+    assert guide.shape[0] == B and guide.shape[2] == Ce
+    L.check(L.load().omg_text_gate(embed.data_ptr(), ld_e, Ce, guide.data_ptr(), guide.shape[1], bias.data_ptr(),
+                                   _ptr(scale), nh, p.data_ptr(), ld_p, out.data_ptr(), ld_o, C2, B, H * W, _stream()),
+            "omg_text_gate")
+    return out
+
+
+def adaptive_maxpool(x, k, out, row0=0):
+    """omg_adaptive_maxpool: AdaptiveMaxPool2d((k, k)) of x (B, H, W, C) (rows may be strided along the channel axis)
+    into rows row0 .. row0 + k*k - 1 of out (B, rows, C) fp16 (unit channel stride)."""
+    _chk16(x)
+    _chk16(out)
+    B, H, W, ldx = _rows(x)
+    Cc = x.shape[3]
+    assert out.dim() == 3 and out.shape[0] == B and out.shape[2] == Cc and out.stride(2) == 1
+    L.check(L.load().omg_adaptive_maxpool(x.data_ptr(), ldx, B, H, W, Cc, k, out.data_ptr(), out.stride(0), out.stride(1),
+                                          row0, _stream()), "omg_adaptive_maxpool")
+    return out
+
+
+def yolo_detect(levels, text, normalize_x, rows=None, nms=None):
+    """omg_yolo_detect for one image.  levels: list of (stride, box (1, fh, fw, >=64) fp16, emb (1, fh, fw, >=E) fp16,
+    cls_scale, cls_bias) with row-major pixels; text fp32 [nc, E] normalised.  Returns (rows [anchors, 6] fp32,
+    detections [n, 6] fp32 or None).  nms: dict(conf, iou, max_wh, agnostic, max_det, gain, pad, clip) or None for
+    pass (a) only."""
+    assert text.is_cuda and text.dtype == torch.float32 and text.is_contiguous() and text.dim() == 2
+    d = L.YoloDesc()
+    d.n_levels, d.nc, d.E, d.normalize_x = len(levels), text.shape[0], text.shape[1], int(bool(normalize_x))
+    T = 0
+    for i, (s, box, emb, sc, bi) in enumerate(levels):
+        _chk16(box)
+        _chk16(emb)
+        B, fh, fw, box_ld = _rows(box)
+        assert B == 1 and emb.shape[:3] == box.shape[:3]
+        d.box[i], d.emb[i], d.box_ld[i], d.emb_ld[i] = box.data_ptr(), emb.data_ptr(), box_ld, _rows(emb)[3]
+        d.cls_scale[i], d.cls_bias[i] = float(sc), float(bi)
+        d.stride[i], d.fh[i], d.fw[i] = s, fh, fw
+        T += fh * fw
+    dev = text.device
+    if rows is None:
+        rows = torch.empty((T, 6), dtype=torch.float32, device=dev)
+    assert rows.shape == (T, 6) and rows.is_contiguous()
+    d.text, d.rows = text.data_ptr(), rows.data_ptr()
+    out = count = None
+    if nms is not None:
+        out = torch.empty((max(nms["max_det"], 1), 6), dtype=torch.float32, device=dev)
+        count = torch.zeros(1, dtype=torch.int32, device=dev)
+        d.conf, d.iou, d.max_wh = float(nms["conf"]), float(nms["iou"]), float(nms.get("max_wh", 7680))
+        d.agnostic, d.max_det = int(bool(nms.get("agnostic", False))), int(nms["max_det"])
+        d.gain, (d.pad_x, d.pad_y), (d.clip_w, d.clip_h) = float(nms["gain"]), nms["pad"], nms["clip"]
+        d.out, d.max_out, d.count = out.data_ptr(), out.shape[0], count.data_ptr()
+    L.check(L.load().omg_yolo_detect(C.byref(d), _stream()), "omg_yolo_detect")
+    return rows, None if out is None else out[: int(count.item())]
+
+
 # ------------------------------------------------------------------ weight packing (host, once per model load)
 def pack_conv3x3_weight(w):
     """torch Conv2d weight [N, C, 3, 3] -> [N, 9*C] with K order (ky, kx, c)."""
