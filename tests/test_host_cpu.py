@@ -286,6 +286,19 @@ def test_c_abi_rejects_bad_arguments_before_touching_the_gpu():
     f.n_concepts, f.noise_main, f.latents = 9, 0x1000, 0x1000
     assert "n_concepts=9 out of range" in err(lib.omg_fuse_step(C.byref(f), None))
     assert "bad channel split" in err(lib.omg_groupnorm(fake, 100, None, 0, 1, 16, fake, fake, 1e-5, 0, fake, fake, None))
+    # one past what shared memory holds: the guide of n = 227 prompts at Ce = 256, 8 heads is (227 * 256 + 256) * 4 B,
+    # 1 KB over the 232 448 B opt-in limit (n = 226 fits exactly)
+    n0 = lib.omg_launch_count()
+    assert "n * Ce = 58112 guide floats exceed shared memory" in err(
+        lib.omg_text_gate(fake, 256, 256, fake, 227, fake, None, 8, fake, 256, fake, 256, 256, 1, 64, None))
+    # one anchor past the 17 800 the one-CTA sort holds: 100^2 + 80^2 + 40 x 35 + 1 x 1
+    y = L.YoloDesc()
+    y.n_levels, y.nc, y.E, y.text, y.rows = 4, 80, 512, 0x1000, 0x1000
+    for i, (s, fh, fw) in enumerate([(8, 100, 100), (16, 80, 80), (32, 40, 35), (64, 1, 1)]):
+        y.box[i] = y.emb[i] = 0x1000
+        y.box_ld[i], y.emb_ld[i], y.stride[i], y.fh[i], y.fw[i] = 64, 512, s, fh, fw
+    assert "17801 anchors exceed the 17800" in err(lib.omg_yolo_detect(C.byref(y), None))
+    assert lib.omg_launch_count() == n0
 
 
 def test_c_abi_rejects_misaligned_vector_operands_before_touching_the_gpu():
@@ -312,6 +325,8 @@ def test_c_abi_rejects_misaligned_vector_operands_before_touching_the_gpu():
     gn = lambda name, x1, x2, y, ws: getattr(lib, name)(x1, 64, x2, 32, 1, 16, ok, ok, 1e-5, 0, ws, y, None)  # noqa: E731
     gna = lambda x1, p1, p2, y: lib.omg_groupnorm_apply(x1, 64, p1, 1, ok, 32, p2, 1, 1, 16, ok, ok, 1e-5, 0, ok, y,  # noqa: E731
                                                         None)
+    # MaxSigmoidAttnBlock's gating at Ce = C2 = 256, 8 heads, 2 prompts, one image of 64 pixels
+    gate = lambda e, p, o: lib.omg_text_gate(e, 256, 256, ok, 2, ok, None, 8, p, 256, o, 256, 256, 1, 64, None)  # noqa: E731
     cases = [
         (lambda: lib.omg_pool2d(off8, ok, 1, 4, 4, 8, 3, 2, 1, 0, 1, 1, None), "omg_pool2d: x must be 16 B aligned"),
         (lambda: lib.omg_pool2d(ok, off2, 1, 4, 4, 8, 3, 2, 1, 0, 1, 0, None), "omg_pool2d: y must be 16 B aligned"),
@@ -350,6 +365,13 @@ def test_c_abi_rejects_misaligned_vector_operands_before_touching_the_gpu():
         (lambda: fuse(noise_main=off4), "omg_fuse_step: noise_main must be 8 B"),
         (lambda: fuse(noise_concept=off4), "omg_fuse_step: noise_concept must be 8 B"),
         (lambda: fuse(latents_f16=off2), "omg_fuse_step: latents_f16 must be 4 B"),
+        (lambda: gate(off8, ok, ok), "omg_text_gate: embed must be 16 B"),
+        (lambda: gate(ok, off2, ok), "omg_text_gate: p must be 16 B"),
+        (lambda: gate(ok, ok, off8), "omg_text_gate: out must be 16 B"),
+        (lambda: lib.omg_adaptive_maxpool(off8, 64, 1, 4, 4, 64, 3, ok, 9 * 64, 64, 0, None),
+         "omg_adaptive_maxpool: x must be 16 B"),
+        (lambda: lib.omg_adaptive_maxpool(ok, 64, 1, 4, 4, 64, 3, off2, 9 * 64, 64, 0, None),
+         "omg_adaptive_maxpool: out must be 16 B"),
     ]
     for call, msg in cases:
         n0 = lib.omg_launch_count()

@@ -1,6 +1,7 @@
 """GPU tests of the YOLO-World path: omg_text_gate and omg_adaptive_maxpool against torch fp32, omg_yolo_detect against
-the float64 numpy restatement (oracle/yolo_world.py), and the whole executor at 640 x 640, l scale, v1 and v2, on
-random weights with random BatchNorm statistics against the fp32 oracle."""
+the float64 numpy restatement (oracle/yolo_world.py), and the whole executor (at 640 x 640, l scale, v1 and v2; at a
+letterboxed 384 x 640, v1 at m and v2 at x) on random weights with random BatchNorm statistics against the fp32
+oracle.  The kernels' edges are in test_yolo_world_kernel_edges_gpu.py."""
 import math
 
 import numpy as np
@@ -63,18 +64,33 @@ def test_text_gate_rejects_bad_operands():
         ops.text_gate(torch.zeros(1, 4, 4, 72, device=DEV).half()[..., 4:68], torch.zeros(1, 2, 64, device=DEV), b, 4, p)
 
 
-@pytest.mark.parametrize("H,W", [(80, 80), (20, 20), (7, 11), (40, 13), (3, 3), (2, 5)])
-def test_adaptive_maxpool_matches_torch(H, W):
+def _pool_case(H, W, k=3, C=64, B=2, row0=9, wide=False, id=None):
+    return pytest.param(H, W, k, C, B, row0, wide, id=id or f"{H}x{W}-k{k}-C{C}-B{B}-row{row0}" + ("-wide" if wide else ""))
+
+
+@pytest.mark.parametrize("H,W,k,C,B,row0,wide", [
+    *[_pool_case(H, W, id=f"{H}-{W}") for H, W in [(80, 80), (20, 20), (7, 11), (40, 13), (3, 3), (2, 5)]],
+    *[_pool_case(H, W, k, C, 3, row0) for k in (1, 2, 3, 5) for (H, W) in [(1, 1), (1, 7), (13, 40), (2, 9)]
+      for C, row0 in [(8, 0), (520, 18)]],
+    _pool_case(13, 40, 3, 64, 3, 18, wide=True),
+    _pool_case(2, 9, 5, 520, 3, 0, wide=True),
+])
+def test_adaptive_maxpool_matches_torch(H, W, k, C, B, row0, wide):
+    """Windows that overlap, windows of one pixel and k > H (windows repeat rows); `wide`: an output whose row stride
+    exceeds C and whose batch stride exceeds rows x row stride.  Everything outside the k x k rows keeps its bits."""
     from omg_b200 import ops
-    torch.manual_seed(H * W)
-    B, C, k = 2, 64, 3
+    torch.manual_seed(H * W + k + C)
+    rows = 32 if row0 + k * k <= 32 else row0 + k * k
     x = torch.randn(B, H, W, C + 16, device=DEV).half()[..., 8:8 + C]
-    out = torch.full((B, 32, C), 7.0, device=DEV).half()
-    ops.adaptive_maxpool(x, k, out, row0=9)
+    buf = torch.full((B, rows + (5 if wide else 0), C + (24 if wide else 0)), 7.0, device=DEV).half()
+    out = buf[:, :rows, 8:8 + C] if wide else buf
+    ops.adaptive_maxpool(x, k, out, row0=row0)
     ref = F.adaptive_max_pool2d(x.float().permute(0, 3, 1, 2), (k, k)).flatten(2).transpose(1, 2)
     torch.cuda.synchronize()
-    assert torch.equal(out[:, 9:18].float(), ref)
-    assert (out[:, :9] == 7).all() and (out[:, 18:] == 7).all()
+    assert torch.equal(out[:, row0:row0 + k * k].float(), ref)
+    inside = torch.zeros_like(buf, dtype=torch.bool)
+    (inside[:, row0:row0 + k * k, 8:8 + C] if wide else inside[:, row0:row0 + k * k]).fill_(True)
+    assert (buf[~inside] == 7).all()
 
 
 def _head_inputs(seed, nc, E=64, sizes=((20, 20), (10, 10), (5, 5)), spread=3.0):
@@ -192,6 +208,66 @@ def test_executor_matches_fp32_oracle_at_640(variant):
     print("best IoU per detection:", np.round(best, 4).tolist())
     assert all(b >= 0.99 or t.any() for b, t in zip(best, tie))
     assert np.mean(best >= 0.99) >= 0.9
+
+
+@pytest.mark.parametrize("variant,scale,heads", [(1, "m", [3, 6, 9]), (2, "x", [5, 10])])
+def test_executor_matches_fp32_oracle_on_a_letterboxed_non_square_input(variant, scale, heads):
+    """A 360 x 640 photo letterboxed with auto=True is 384 x 640: grids 48 x 80 / 24 x 40 / 12 x 20.  v1 at m runs the
+    text gate with 3, 6 and 9 heads and ImagePoolingAttn on non-square maps; v2 at x runs 5 and 10 heads.  The head maps
+    against the fp32 oracle, then omg_yolo_detect's rows against the float64 anchor_rows of the executor's own head
+    maps (a grid's height and width swapped on the host would show here), and its detections bit for bit against the
+    float32 NMS restatement of its own rows."""
+    import os
+    import sys
+    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+    from test_yolo_world_kernel_edges_gpu import K_ANCHOR_BOX, K_ANCHOR_SCORE, U32, nms_float32
+    from test_kernel_edges_gpu import check
+    from omg_b200.yolo_world import PackedYoloWorld, box_rescale
+    from oracle import yolo_world as O
+    ref = O.randomize_(O.WorldModel(variant, scale), seed=10 + variant, bias=0.0).to(DEV)
+    assert sorted({s["nh"] for s in ref.layers if s["type"] == "C2fAttn"}) == heads
+    g = torch.Generator().manual_seed(variant)
+    img = torch.rand(1, 3, 384, 640, generator=g)
+    text = F.normalize(torch.randn(1, 3, 512, generator=g), dim=-1)
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    with torch.no_grad():
+        y, raw = ref(img.to(DEV), text.to(DEV))
+        # about 40 anchors above conf = 0.1
+        top = torch.logit(y[0, 4:].max(0)[0].double()).sort(descending=True)[0]
+        for h in ref.model[-1].cv4:
+            h.bias.fill_(math.log(0.1 / 0.9) - float(top[40]))
+        if variant == 2:
+            raw = [(b, h.norm(e)) for (b, e), h in zip(raw, ref.model[-1].cv4)]
+    raw = [(b.cpu(), e.cpu()) for b, e in raw]
+    assert [tuple(b.shape[2:]) for b, _ in raw] == [(48, 80), (24, 40), (12, 20)]
+    packed = PackedYoloWorld(ref.state_dict(), device=DEV)
+    x = torch.zeros(1, 384, 640, 8)
+    x[..., :3] = img[0].permute(1, 2, 0)
+    x = x.half().to(DEV)
+    lv = packed.forward(x, text.to(DEV))
+    worst = [(_rel(b[0].float().cpu(), rb[0].permute(1, 2, 0)), _rel(e[0].float().cpu(), re[0].permute(1, 2, 0)))
+             for (b, e), (rb, re) in zip(lv, raw)]
+    print("rel-L2 per level (box, emb):", worst)
+    assert max(w[0] for w in worst) <= TOL_BOX and max(w[1] for w in worst) <= TOL_EMB
+    gain, pad = box_rescale((384, 640), (360, 640))
+    nms = {"conf": 0.1, "iou": 0.7, "agnostic": False, "max_det": 300, "gain": gain, "pad": pad, "clip": (640.0, 360.0)}
+    rows, det = packed.detect(x, text.to(DEV), nms)
+    head = packed.packs[-1]
+    tn = text[0].float()
+    tn = tn / tn.norm(dim=-1, keepdim=True).clamp_min(1e-12)    # as detect() normalises the prompts
+    want = O.anchor_rows([b[0].cpu().numpy() for b, _ in lv], [e[0].cpu().numpy() for _, e in lv], tn.numpy(),
+                         (8, 16, 32), [p["scale"] for p in head["levels"]], [p["bias"] for p in head["levels"]],
+                         head["normalize_x"])
+    want = torch.from_numpy(want)
+    got = rows.cpu().double()
+    check(got[:, :4], want[:, :4], K_ANCHOR_BOX, u=U32, what=f"v{variant}-{scale} anchor boxes")
+    check(got[:, 4], want[:, 4], K_ANCHOR_SCORE, u=U32, what=f"v{variant}-{scale} anchor scores")
+    assert (got[:, 5] == want[:, 5]).double().mean() >= 0.999
+    kept, ref_det = nms_float32(rows.cpu().numpy(), **nms)
+    det = det.cpu().numpy()
+    print(f"v{variant}-{scale}: {len(det)} detections")
+    assert len(det) == len(ref_det) > 0
+    assert np.array_equal(det.view(np.uint32), ref_det.view(np.uint32))
 
 
 def test_yolo_world_surface_and_best_box():
