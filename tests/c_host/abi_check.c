@@ -9,12 +9,15 @@ int main(void) {
     omg_gemm_desc g;
     omg_attn_desc a;
     omg_fuse_desc f;
+    omg_solver_desc s;
     omg_plan* p = 0;
     (void)g;
     (void)a;
     (void)f;
+    (void)s;
     (void)p;
-    printf("%u %u %u %u %u\n", (unsigned)sizeof(omg_view4), (unsigned)sizeof(omg_seg), (unsigned)sizeof(omg_gemm_desc),
-           (unsigned)sizeof(omg_attn_desc), (unsigned)sizeof(omg_fuse_desc));
+    printf("%u %u %u %u %u %u\n", (unsigned)sizeof(omg_view4), (unsigned)sizeof(omg_seg),
+           (unsigned)sizeof(omg_gemm_desc), (unsigned)sizeof(omg_attn_desc), (unsigned)sizeof(omg_fuse_desc),
+           (unsigned)sizeof(omg_solver_desc));
     return 0;
 }

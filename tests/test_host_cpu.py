@@ -50,7 +50,8 @@ def test_header_is_plain_c99_and_matches_the_ctypes_layout():
         subprocess.run([cc, "-std=c99", "-pedantic", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
                         os.path.join(ROOT, "tests", "c_host", "abi_check.c"), "-o", exe], check=True)
         sizes = [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
-    assert sizes == [ctypes.sizeof(t) for t in (L.View4, L.Seg, L.GemmDesc, L.AttnDesc, L.FuseDesc)]
+    assert sizes == [ctypes.sizeof(t) for t in (L.View4, L.Seg, L.GemmDesc, L.AttnDesc, L.FuseDesc,
+                                                           L.SolverDesc)]
 
 
 def test_launch_plan_handle_protocol():

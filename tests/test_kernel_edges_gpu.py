@@ -23,7 +23,8 @@ PAD = 8  # elements; a multiple of 8 keeps the kernels' 16 B row alignment
 # Per-element k of each kernel family, with the worst value the family's cases need on an NVIDIA H100 80GB HBM3 at a
 # 400 W power limit (a value <= 0 means every element is already within 4 u |ref|).
 K_GEMM = 1.0      # measured 0.00 (GEMM, convs, weight planes)
-K_F32 = 32.0      # fp32 results, u = 2^-24: measured 17.4 (out_f32, 320-wide tiles), 7.7 (fuse_step latents)
+K_F32 = 32.0      # fp32 results, u = 2^-24: measured 17.4 (out_f32, 320-wide tiles), 7.7 (fuse_step latents);
+                  # the same Euler step through solver_step needs 1.9 (H100 80GB HBM3 at 700 W)
 K_ATTN = 4.0      # measured 1.6 (16 items, n_kv = 77)
 K_NORM = 1.0      # measured 0.23 (GroupNorm from omg_colstats at |mean| / sigma = 32)
 K_ELEM = 1.0      # measured 0.00
@@ -618,12 +619,15 @@ def test_ctx_mix(ops, Lk, C):
     check(out, torch.einsum("wn,bnc->bwc", coef.double(), ctx.double()), K_ELEM, what=f"ctx_mix L={Lk} C={C}")
 
 
+@pytest.mark.parametrize("kernel", ["fuse", "solver"])
 @pytest.mark.parametrize("next_inputs", ["both", "main_only", "concept_only"])
 @pytest.mark.parametrize("HW", [1, 129, 4097])
-def test_fuse_step_eight_concepts(ops, HW, next_inputs):
+def test_fuse_step_eight_concepts(ops, HW, next_inputs, kernel):
     """8 concepts: overlapping masks, two concepts without a mask (skipped), a 0.5-valued stripe (outside the mask, as in
     the reference's `mask == 1` selection); NaN in channels 4..7 of every noise row must reach no output; the fp16
-    latent copy is the fp32 state rounded; a NULL next-input pointer leaves its buffer untouched."""
+    latent copy is the fp32 state rounded; a NULL next-input pointer leaves its buffer untouched.  The same Euler step
+    runs through omg_fuse_step and through omg_solver_step with Euler's coefficients (no history, no noise)."""
+    from omg_b200.scheduler import StepCoeffs
     gen = torch.Generator(device="cuda").manual_seed(HW)
 
     def noise(rows):
@@ -651,8 +655,13 @@ def test_fuse_step_eight_concepts(ops, HW, next_inputs):
         lat.before = lat.buf.clone()
         l16 = Guard((2, HW, 4), flat=True)
         nxt, nxc = Guard((4, HW, 8), flat=True), Guard((2, HW, 8), flat=True)
-        ops.fuse_step(nm, ncs, masks, gs, sig, sign, lat.out, nxt.out if next_inputs != "concept_only" else None,
-                      nxc.out if next_inputs != "main_only" else None, latents_f16=l16.out)
+        nxt_p = nxt.out if next_inputs != "concept_only" else None
+        nxc_p = nxc.out if next_inputs != "main_only" else None
+        if kernel == "fuse":
+            ops.fuse_step(nm, ncs, masks, gs, sig, sign, lat.out, nxt_p, nxc_p, latents_f16=l16.out)
+        else:
+            k = StepCoeffs(1.0, -sig, sign / sig, 1.0 - sign / sig, 0.0, 0.0, 1.0 / math.sqrt(sign * sign + 1))
+            ops.solver_step(nm, ncs, masks, gs, k, lat.out, nxt_p, nxc_p, l16.out)
         torch.cuda.synchronize()
         assert lat.intact() and l16.intact() and nxt.intact() and nxc.intact()
         return [lat.out.clone(), l16.out.clone(), nxt.out.clone(), nxc.out.clone()]
@@ -671,16 +680,16 @@ def test_fuse_step_eight_concepts(ops, HW, next_inputs):
             new[1] = new[1] + s * ncs[k][1, :, :4].double()
     eps = torch.stack([n[0] + gs * (n[2] - n[0]), new[0] + gs * (new[1] - new[0])])
     ref = lat0.double() + eps * (sign - sig)
-    check(lat, ref, K_F32, rel_l2=1e-6, u=2.0 ** -24, what=f"fuse_step latents HW={HW}")
+    check(lat, ref, K_F32, rel_l2=1e-6, u=2.0 ** -24, what=f"{kernel}_step latents HW={HW}")
     assert same_bits(l16, lat.half())
     sc = ref / math.sqrt(sign * sign + 1)
     if next_inputs != "concept_only":
-        check(nxt[..., :4], torch.cat([sc, sc]), K_ELEM, what="fuse_step next_main_in")
+        check(nxt[..., :4], torch.cat([sc, sc]), K_ELEM, what=f"{kernel}_step next_main_in HW={HW}")
         assert (_bits(nxt[..., 4:]) == 0).all()
     else:
         assert torch.isnan(nxt).all()
     if next_inputs != "main_only":
-        check(nxc[..., :4], torch.stack([sc[1], sc[1]]), K_ELEM, what="fuse_step next_concept_in")
+        check(nxc[..., :4], torch.stack([sc[1], sc[1]]), K_ELEM, what=f"{kernel}_step next_concept_in HW={HW}")
         assert (_bits(nxc[..., 4:]) == 0).all()
     else:
         assert torch.isnan(nxc).all()

@@ -14,38 +14,11 @@ import torch
 
 from omg_b200 import scheduler as S
 import util_schedulers as O  # noqa: E402
+from util_schedulers import configs  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = S.SDXL_BASE_CONFIG
 STEPS = (2, 3, 14, 15, 16, 20, 25, 30, 50)
-
-
-def configs():
-    """Every supported rule (name, schedule) over the three spacings, built from SDXL-base's config as users do."""
-    out = []
-    for sp in ("leading", "trailing", "linspace"):
-        for k in (False, True):
-            for pt in ("epsilon", "v_prediction"):
-                out.append((f"euler-{sp}-karras{int(k)}-{pt}",
-                            S.EulerDiscreteScheduler.from_config(BASE, timestep_spacing=sp, use_karras_sigmas=k,
-                                                                 prediction_type=pt)))
-        for pt in ("epsilon", "v_prediction"):
-            out.append((f"euler_a-{sp}-{pt}",
-                        S.EulerAncestralDiscreteScheduler.from_config(BASE, timestep_spacing=sp, prediction_type=pt)))
-        for k in (False, True):
-            for alg in ("dpmsolver++", "sde-dpmsolver++"):
-                for st in ("midpoint", "heun"):
-                    for pt in ("epsilon", "v_prediction"):
-                        out.append((f"dpm-{sp}-karras{int(k)}-{alg}-{st}-{pt}",
-                                    S.DPMSolverMultistepScheduler.from_config(
-                                        BASE, timestep_spacing=sp, use_karras_sigmas=k, algorithm_type=alg,
-                                        solver_type=st, prediction_type=pt)))
-    out.append(("dpm-order1", S.DPMSolverMultistepScheduler.from_config(BASE, solver_order=1)))
-    out.append(("dpm-no-lower-order-final", S.DPMSolverMultistepScheduler.from_config(BASE, lower_order_final=False)))
-    out.append(("dpm-euler-at-final", S.DPMSolverMultistepScheduler.from_config(BASE, euler_at_final=True)))
-    out.append(("euler-linear-betas", S.EulerDiscreteScheduler.from_config(BASE, beta_schedule="linear",
-                                                                           beta_start=0.0001, beta_end=0.02)))
-    return out
 
 
 CONFIGS = configs()

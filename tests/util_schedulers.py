@@ -2,7 +2,8 @@
 literally in torch [third-party recollection; omg_b200/scheduler.py lists what it rests on].  TEST INFRASTRUCTURE: the
 step() arithmetic as diffusers writes it, float32 tables, the sample's dtype for the arithmetic, indexed by the step
 index i instead of the timestep.  The tests check omg_b200/scheduler.py's coefficient form against these classes, and
-run oracle.pipeline.denoise with one of them in place of its default Euler (`oracle_schedule`)."""
+run oracle.pipeline.denoise with one of them in place of its default Euler (`oracle_schedule`).  `configs()` lists the
+host schedules every supported rule gives, for the CPU and kernel tests alike."""
 import contextlib
 
 import numpy as np
@@ -238,6 +239,37 @@ def make(cls_name: str, config: dict, noise_source=None):
     return {"EulerDiscreteScheduler": EulerDiscreteScheduler,
             "EulerAncestralDiscreteScheduler": EulerAncestralDiscreteScheduler,
             "DPMSolverMultistepScheduler": DPMSolverMultistepScheduler}[cls_name](noise_source, **config)
+
+
+def configs():
+    """Every supported rule (name, host schedule) over the three spacings, built from SDXL-base's config as users do.
+    The one function here that uses omg_b200.scheduler: the restatements above stay independent of it."""
+    from omg_b200 import scheduler as S
+    BASE = S.SDXL_BASE_CONFIG
+    out = []
+    for sp in ("leading", "trailing", "linspace"):
+        for k in (False, True):
+            for pt in ("epsilon", "v_prediction"):
+                out.append((f"euler-{sp}-karras{int(k)}-{pt}",
+                            S.EulerDiscreteScheduler.from_config(BASE, timestep_spacing=sp, use_karras_sigmas=k,
+                                                                 prediction_type=pt)))
+        for pt in ("epsilon", "v_prediction"):
+            out.append((f"euler_a-{sp}-{pt}",
+                        S.EulerAncestralDiscreteScheduler.from_config(BASE, timestep_spacing=sp, prediction_type=pt)))
+        for k in (False, True):
+            for alg in ("dpmsolver++", "sde-dpmsolver++"):
+                for st in ("midpoint", "heun"):
+                    for pt in ("epsilon", "v_prediction"):
+                        out.append((f"dpm-{sp}-karras{int(k)}-{alg}-{st}-{pt}",
+                                    S.DPMSolverMultistepScheduler.from_config(
+                                        BASE, timestep_spacing=sp, use_karras_sigmas=k, algorithm_type=alg,
+                                        solver_type=st, prediction_type=pt)))
+    out.append(("dpm-order1", S.DPMSolverMultistepScheduler.from_config(BASE, solver_order=1)))
+    out.append(("dpm-no-lower-order-final", S.DPMSolverMultistepScheduler.from_config(BASE, lower_order_final=False)))
+    out.append(("dpm-euler-at-final", S.DPMSolverMultistepScheduler.from_config(BASE, euler_at_final=True)))
+    out.append(("euler-linear-betas", S.EulerDiscreteScheduler.from_config(BASE, beta_schedule="linear",
+                                                                           beta_start=0.0001, beta_end=0.02)))
+    return out
 
 
 @contextlib.contextmanager
